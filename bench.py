@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- stylized frames/s at 1280x720 (BASELINE.json metric), one JSON line on stdout.
 
-  python bench.py --gpus N --steps K --warmup W          # this implementation (libfav_b200.so, sm_100a)
+  python bench.py --gpus N --steps K --warmup W          # this implementation (libfav_b200.so, sm_90a)
   python bench.py --impl reference --gpus N ...           # the reference's CPU nn path (oracle port) on host cores
 
 A "step" = ONE FRAME of the hot path: fused warp+mask+preprocess+concat -> 7-channel input -> stylization net ->
@@ -13,7 +13,7 @@ architecture: no network => no released checkpoints), synthetic frames / flows /
   e2e        frames/s through the host-buffer session API (fav_session_*): every step copies the frame, the
              backward+forward flow from PINNED host memory, computes the occlusion mask on the GPU, and reads
              the stylized frame back to pinned host memory -- all inside the timed region
-  roofline   dominant kernel = conv_tc_kernel (tcgen05 implicit GEMM): algorithmic FLOPs / CUDA-event time
+  roofline   dominant kernel = conv_tc_kernel (wgmma implicit GEMM): algorithmic FLOPs / CUDA-event time
   roofline_front  the fused temporal-input kernel (warp-kernel HBM GB/s of the metric), 64 B/px
   cpu_baseline    the oracle port (PyTorch-CPU fp32 restatement + C front end) on the box's host cores
 N > 1: one process per GPU (torchrun), independent clips (replicas, weak scaling); NCCL only broadcasts the input
@@ -41,12 +41,9 @@ import torch  # noqa: E402
 H, W = 720, 1280
 ARCHS = {"default": "c9s1-32,d64,d128,R128,R128,R128,R128,R128,u64,u32,c9s1-3",
          "paper": "c9s1-32,d64,d128,R128,R128,R128,R128,R128,U2,c3s1-64,U2,c9s1-3"}
-POOL = 8  # distinct input frames cycled: 8 x 29.5 MB of inputs per rank > 126 MB L2
+POOL = 8  # distinct input frames cycled: 8 x 29.5 MB of inputs per rank > 50 MB L2
 CONV_GFLOP_720P = 274.3  # SURVEY.md 8(d): logical-channel conv FLOPs per 720p frame, default arch (variant u)
 FRONT_BYTES_PER_PX = 64  # fused temporal-input kernel, all-fp32 I/O (SURVEY.md 8(d))
-NCU_RES_CONV_DRAM_BYTES = 34215000 + 1113000  # mean of the 10 residual conv_res_kernel launches of one frame, ncu --set full (profiles/r02_frame_raw.csv.gz)
-NCU_FRONT_DRAM_BYTES = 33185280 + 586240      # temporal_input_kernel @720p (profiles/r02_frame_raw.csv.gz)
-NCU_STAGE_DRAM_BYTES = 37158400 + 1045760      # temporal_stage_kernel<1,0> @720p (profiles/r02_frame_raw.csv.gz)
 
 
 WORKLOAD = "1280x720 clip (BASELINE.json configs[1]), candy (seeded random-init weights), one step = one frame of run_next_image"
@@ -63,7 +60,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16")
 
 
 class ClockSampler:
@@ -240,11 +237,8 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item())
 
-    # Timed regions: each is EXACTLY K steps bracketed by barrier + synchronize; regions repeat until >= 1 s of device time
-    # has been measured (so that short driver runs still amortise pipeline fill and give the clock sampler samples) and the
-    # MEDIAN region is reported.
-    def n_regions(t_first):
-        return max(1, min(60, int(1.0 / max(t_first, 1e-4)) + 1))
+    # Timed regions: each is EXACTLY K steps bracketed by barrier + synchronize, one region per figure, so --steps is the
+    # number of timed steps of the reported path.
 
     sampler = ClockSampler(local)
     if rank == 0:
@@ -275,14 +269,13 @@ def run_ours(args):
         barrier()
         return max_over_ranks(e0.elapsed_time(e1) / 1e3), int(_lib.lib.fav_launch_count() - l0)
 
-    t_first, launches = region_dev(False)
-    regions = n_regions(t_first)
-    t_list = sorted([t_first] + [region_dev(False)[0] for _ in range(regions - 1)])
-    t_dev = t_list[len(t_list) // 2]
+    t_dev, launches = region_dev(False)
     checksum = float(prev.double().sum().item())
+    if args.dump_outputs and rank == 0:  # what the timed path returned in its last step (3 x 720 x 1280 fp32, 11 MB)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "stylized.npy"), prev.float().cpu().numpy())
     value = world * K / t_dev
-    tf_list = sorted(region_dev(True)[0] for _ in range(regions))
-    t_full = tf_list[len(tf_list) // 2]
+    t_full = region_dev(True)[0]
     value_full = world * K / t_full
 
     # ---- (2) end to end through the host-buffer API ------------------------------------------------------------
@@ -308,8 +301,7 @@ def run_ours(args):
         barrier()
         return max_over_ranks(time.perf_counter() - t0), t_enq
 
-    e_list = sorted(region_e2e() for _ in range(regions))
-    t_e2e, t_enqueue = e_list[len(e_list) // 2]
+    t_e2e, t_enqueue = region_e2e()
     tw1 = time.time()
     clocks = sampler.stop(tw0, tw1) if rank == 0 else None
     gpu_ms_last = sess.last_gpu_ms()
@@ -368,7 +360,7 @@ def run_ours(args):
         _lib.dptr(out7), None, H, W, 7, 0, _lib.stream_ptr())))
     stage_gbs = 68 * H * W / (stage_ms * 1e-3) / 1e9
     # (c) standalone warp op (metric half 2: warp-kernel HBM GB/s, 32 B/px) and the kernel to beat: the reference's own CUDA
-    # kernel compiled for sm_100a (oracle/_ref/libref_warp.so, original 32x16 blocks), same inputs, real and stress flows
+    # kernel compiled for sm_90a (oracle/_ref/libref_warp.so, original 32x16 blocks), same inputs, real and stress flows
     warp = {}
     if rank == 0:
         from oracle import refwarp
@@ -403,16 +395,16 @@ def run_ours(args):
         line = {
             "metric": "stylized frames/sec at 1280x720", "value": value, "value_full": value_full, "unit": "frames/s", "n_gpus": world,
             "steps": K, "warmup": Wm, "ms_per_step": 1e3 * t_dev / K, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": "f16x2 (fp16 hi/lo operand pairs, 3 tcgen05 MMAs per product, fp32 accumulate)",
+            "vs_baseline": None, "dtype": "f16x2 (fp16 hi/lo operand pairs, 3 wgmma MMAs per product, fp32 accumulate)",
             "data": "synthetic",
             "config": config_for(args.arch),
-            "notes": {"l2": f"inputs cycle through a pool of {POOL} distinct frames ({POOL * 29.5:.0f} MB > 126 MB L2); "
+            "notes": {"l2": f"inputs cycle through a pool of {POOL} distinct frames ({POOL * 29.5:.0f} MB > 50 MB L2); "
                             "~1.5 GB of activations stream through L2 per frame",
                       "parallelism": f"replicas x{world} (independent clips, no data-path collective)",
                       "precision": "outputs within 1e-3 of the fp64 oracle (measured ~1e-5, tests/test_gpu_net.py, "
                                    "tests/test_gpu_parity_large.py)",
-                      "timing": f"{regions} timed regions of exactly {K} steps each (barrier + synchronize on both sides, CUDA "
-                                "events, max over ranks); value / e2e = the MEDIAN region"},
+                      "timing": f"one timed region of exactly {K} steps per figure (barrier + synchronize on both sides, CUDA "
+                                "events, max over ranks)"},
             "e2e": {"value": e2e, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": 1e3 * t_e2e / K, "host_enqueue_ms_per_step": 1e3 * t_enqueue / K,
                     "gpu_ms_last_frame": gpu_ms_last,
@@ -422,12 +414,10 @@ def run_ours(args):
             "clocks": clocks,
             "host": {"gpu_numa_binding": numa},
             "roofline": {"bound": "tensor",
-                         "kernel": "conv_res_kernel, residual-block launches (128->128 3x3; 10 of the %d conv launches per " % n_conv_launch +
+                         "kernel": "conv_tc_kernel, residual-block launches (128->128 3x3; 10 of the %d conv launches per " % n_conv_launch +
                                    "frame, the largest share of the step; the second conv of each block also normalises its input on load)",
                          "achieved": res_tfs, "peak": pk["tf_sust"], "unit": "TFLOP/s", "frac": res_tfs / pk["tf_sust"],
-                         "traffic": NCU_RES_CONV_DRAM_BYTES,
-                         "traffic_source": "profiles/r02_frame_raw.csv.gz (dram__bytes_read.sum + dram__bytes_write.sum, mean of the 10 "
-                                           "launches of one frame; algorithmic bytes per launch 68.5 MB: the planar raw output stays in L2)",
+                         "traffic": None,
                          "peak_source": pk["src"] + ", bf16 sustained (kernel timed inside the step)",
                          "algorithmic_flop_per_launch": res_flop / max(1, res_n), "us_per_launch": 1e3 * res_ms / max(1, res_n),
                          "launches_timed": res_n,
@@ -439,15 +429,11 @@ def run_ours(args):
             "roofline_stage": {"bound": "hbm", "kernel": "temporal_stage_kernel<false,0> (the whole temporal stage in one launch: "
                                "occlusion test from the flow pair + 7x7 min filter + warp + mask + preprocess + concat)",
                                "achieved": stage_gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": stage_gbs / pk["hbm"],
-                               "bytes_per_launch": 68 * H * W, "ms": stage_ms, "traffic": NCU_STAGE_DRAM_BYTES,
-                               "traffic_source": "profiles/r02_frame_raw.csv.gz (37.2 MB read = the input planes; the packed operand it "
-                                                 "writes stays in L2); not memory bound: the occlusion test's mixed float/double chain",
+                               "bytes_per_launch": 68 * H * W, "ms": stage_ms, "traffic": None,
                                "timing": f"{nf} launches in one CUDA graph, inputs cycle through {POOL} frames, best of 5 replays"},
             "roofline_front": {"bound": "hbm", "kernel": "temporal_input_kernel (fused warp+mask+preprocess+concat)",
                                "achieved": front_gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": front_gbs / pk["hbm"],
-                               "traffic": NCU_FRONT_DRAM_BYTES,
-                               "traffic_source": "profiles/r02_frame_raw.csv.gz (33.2 MB read = exactly the input planes; "
-                                                 "the 25.8 MB written stay in the 126 MB L2)",
+                               "traffic": None,
                                "bytes_per_launch": FRONT_BYTES_PER_PX * H * W, "ms": front_ms},
             "roofline_warp": None if not warp else {
                 "bound": "hbm", "kernel": "warp_vec4_kernel<3> via fav_warp_image (nn.BilinearSamplerBDHW forward, 3x720x1280)",
@@ -455,7 +441,7 @@ def run_ours(args):
                 "bytes_per_launch": 32 * H * W, "traffic": None,
                 "vs_original_kernel": warp["real"]["vs_original_kernel"],
                 "real_flow": warp["real"], "stress_flow_u64px": warp["stress"],
-                "original_kernel": "stnbdhw/BilinearSamplerBDHW.cu:48-109 compiled for sm_100a from /root/reference "
+                "original_kernel": "stnbdhw/BilinearSamplerBDHW.cu:48-109 compiled for sm_90a from the reference sources "
                                    "(oracle/Makefile refwarp), launch config of :119-120"},
             "value_full_note": "value_full = device-resident frames/s with the occlusion test (flow pair) and the 7x7 min filter "
                                "inside the timed region as well (the whole north-star path; `value` takes precomputed certainty)",
@@ -620,7 +606,7 @@ def run_cfg3(args):
         line = {"metric": "stylized frames/sec, 8 independent 1920x1080 clips (BASELINE.json configs[2])", "value": NC * F / t_max,
                 "unit": "frames/s", "n_gpus": world, "steps": F, "warmup": 2 * CH, "ms_per_step": 1e3 * t_max / F,
                 "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-                "dtype": "f16x2 (fp16 hi/lo operand pairs, 3 tcgen05 MMAs per product, fp32 accumulate)", "data": "synthetic",
+                "dtype": "f16x2 (fp16 hi/lo operand pairs, 3 wgmma MMAs per product, fp32 accumulate)", "data": "synthetic",
                 "config": {"workload": "8 x 1920x1080 clips, candy (synthetic weights), one step = one frame of EVERY clip",
                            "arch": ARCHS[args.arch], "frames_per_clip": F, "chunk": CH,
                            "parallelism": f"clips round-robin over {world} GPU(s); rank 0 scatters inputs / gathers outputs (NCCL p2p)"},
@@ -650,6 +636,8 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=300)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the stylized frame of the last timed step as DIR/stylized.npy (float32)")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--config", default="cfg2", choices=["cfg2", "cfg3"],

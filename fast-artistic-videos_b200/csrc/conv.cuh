@@ -9,7 +9,7 @@ constexpr int kMaxSteps = 168;
 constexpr int kMaxRfRows = 24;  // row-fold: R + KH - 1 patch rows per unit
 constexpr int kMaxRows = 10;
 constexpr int kMaxGroups = 12;
-constexpr int kTileM = 128;  // output pixels per MMA tile = TMEM lanes
+constexpr int kTileM = 128;  // output pixels per tile (two 64-row wgmma halves)
 constexpr int kTraceWords = 64;   // u64 words per CTA in the optional timeline buffer
 constexpr int kTraceUnits = 6;    // units (tiles) per CTA recorded
 
@@ -22,7 +22,7 @@ struct KStep {
   uint16_t lbo16;
 };
 
-// tcgen05 implicit-GEMM job (one convolution, or one sub-pixel phase of a transposed convolution)
+// tensor-core (wgmma) implicit-GEMM job (one convolution, or one sub-pixel phase of a transposed convolution)
 struct ConvJob {
   // input operand (hi/lo fp16 planes), addressed in 16-byte units
   const uint4 *a_hi, *a_lo;
@@ -52,7 +52,7 @@ struct ConvJob {
   int b_slots, b_resident;
   int a_stages;  // patch pipeline depth (2..4), chosen from the shared-memory budget
   // mt: output rows per work unit (1 or 2).  mt = 2 shares every weight chunk and the overlapping patch rows between
-  // two vertically adjacent 128-pixel tiles (M = 256, two TMEM accumulators): halves the weight traffic per pixel.
+  // two vertically adjacent 128-pixel tiles (M = 256, two accumulators): halves the weight traffic per pixel.
   int mt;
   // row-fold (tall filters with a narrow N block: conv1 9x9 7->32, x-folded final 9x9): a unit is rf_R output rows;
   // the patch is walked row by row and the MMA of patch row iy accumulates into ALL output rows r with
@@ -80,7 +80,7 @@ struct ConvJob {
   // per-CTA timeline (diagnostics, fav_debug_set_trace): kTraceWords u64 per CTA, null = off.  Layout in conv_tc.cu.
   unsigned long long *trace;
   // timing ablations (env FAV_DBG, diagnostics only; results are wrong when non-zero): 1 = no epilogue stores/stats,
-  // 2 = 16-byte weight copies, 4 = 16-byte patch copies, 8 = epilogue skips the TMEM loads too
+  // 2 = 16-byte weight copies, 4 = 16-byte patch copies, 8 = no epilogue at all
   int dbg;
   // fused InstanceNorm statistics: per-channel sum / sum of squares of the stored values (double, atomics), or null
   double *stats;
@@ -106,7 +106,7 @@ struct SimtJob {
   int Ho, Wo;
   float *raw;
   int raw_Cq, raw_Wp;
-  int raw_planar, raw_Hp;  // planar raw output [C][Hp][Wp] (steps whose tcgen05 path is conv_res.cu)
+  int raw_planar, raw_Hp;  // planar raw output [C][Hp][Wp] (CUDA-core comparator only)
   int oy_mul, oy_off, ox_mul, ox_off;
   int final_mode;
   float *out3;

@@ -1,4 +1,4 @@
-// conv_plan.hpp -- host-only planning of the tcgen05 implicit-GEMM convolution: filter-tap tables, K-step
+// conv_plan.hpp -- host-only planning of the wgmma implicit-GEMM convolution: filter-tap tables, K-step
 // tables, weight packing and operand geometry.  Pure functions without CUDA runtime calls so that the same
 // code is exercised on the CPU by tests/emu (an emulation of the kernel's addressing) and on the GPU by net.cu.
 #pragma once
@@ -59,6 +59,10 @@ struct ConvDef {
 // ---- tcgen05 tables for one phase -------------------------------------------------------------------------
 static constexpr int kStageCapBytes = 56 * 1024;  // one A stage (hi + lo)
 static constexpr int kChunkCapBytes = 24 * 1024;
+// conv_tc.cu (wgmma) keeps one register accumulator of Npad columns per 64-pixel half-tile.  The row-fold and phase-fold
+// plans write per-row / per-phase column ranges of one wide accumulator, two-row units and the K-split need a second
+// accumulator: none of them is planned.
+static constexpr bool kPlanRowFold = false, kPlanPhaseFold = false;
 
 static inline int build_phase_tables(const ConvDef &c, ConvPhase &ph) {
   ph.rows.clear();
@@ -107,8 +111,6 @@ static inline int build_phase_tables(const ConvDef &c, ConvPhase &ph) {
       return FAV_ERR_UNSUPPORTED;
     }
     ph.kind = 0; ph.CbG = (c.Cb % 4 == 0) ? 4 : 2;
-    // 3x3 stride-1 layers with 128 output channels run on conv_res.cu, whose stages hold two channel blocks
-    if (c.k == 3 && c.stride == 1 && c.cout == 128 && !c.transposed) ph.CbG = 2;
     if (const char *e = getenv("FAV_CBG")) { int v = atoi(e); if (v == 2 || v == 4) ph.CbG = v; }  // tuning knob
     ph.nchg = c.Cb / ph.CbG;
     ph.nseg = 1; ph.pslab16 = kTileM + (ph.dxmax - ph.dxmin); ph.seg_len16[0] = ph.pslab16; ph.seg_dst16[0] = 0;
@@ -167,7 +169,7 @@ static inline int build_phase_tables(const ConvDef &c, ConvPhase &ph) {
   }
   // ---- row-fold for tall filters with a narrow N block (see conv.cuh) -------------------------------------------
   ph.rf_R = 0;
-  if ((ph.kind == 1 || ph.kind == 3) && !c.transposed && c.in_stride == 1 && nrows >= 5 && ph.Npad <= 32 &&
+  if (kPlanRowFold && (ph.kind == 1 || ph.kind == 3) && !c.transposed && c.in_stride == 1 && nrows >= 5 && ph.Npad <= 32 &&
       nrows * ph.Npad <= 512 && c.Cb <= 4) {  // Cb = 8 (64-channel final conv of the paper arch): a 35 KB patch row per
                                               // stage leaves 12 MMAs per stage -- latency bound, 359 us vs 156 us unfolded (measured)
     const int saveCbG = ph.CbG, saveNchg = ph.nchg;
@@ -323,7 +325,7 @@ static inline void build_phases(ConvDef &c) {
         }
         c.phases.push_back(std::move(ph));
       }
-    c.has_fold = build_phase_fold(c, c.fold) == FAV_OK;
+    c.has_fold = kPlanPhaseFold && build_phase_fold(c, c.fold) == FAV_OK;
   }
 }
 
@@ -428,13 +430,7 @@ static inline int fill_conv_job(const ConvDef &c, const ConvPhase &ph, const Ope
   j.a_Cb = in.Cb; j.a_slab16 = in.slab16();
   j.tile_dx = ph.kind == 3 ? kTileM - (c.k - 1) : kTileM;
   j.xfold_kw = ph.kind == 3 ? c.k : 0;
-  // two rows per unit when the weights do not fit in shared memory (they would be re-streamed per tile) and the
-  // patch rows are consecutive input rows
-  const size_t total_b = (size_t)ph.nrg * ph.nchg * ph.steps.size() * 2 * 2 * ph.Npad * 16;
-  bool consecutive = ph.kind == 0 && c.in_stride == 1 && ph.nrg == 1;
-  for (size_t i = 1; i < ph.rows.size(); ++i) consecutive = consecutive && ph.rows[i] == ph.rows[i - 1] + 1;
-  j.mt = (consecutive && total_b > 160 * 1024 && ph.Npad * 2 * 2 <= 512 &&
-          (size_t)(ph.rows_per_group + 1) * ph.CbG * ph.pslab16 * 32 <= 72 * 1024 && pHo >= 2) ? 2 : 1;
+  j.mt = 1;  // one output row per unit (see kPlanRowFold)
   if (ph.rf_R) j.mt = ph.rf_R;
   if (ph.pf) j.mt = 1;
   j.Ho = pHo; j.Wo = pWo; j.tiles_x = ceil_div(pWo, j.tile_dx); j.ntiles = j.tiles_x * ceil_div(pHo, j.mt);
@@ -479,13 +475,7 @@ static inline int fill_conv_job(const ConvDef &c, const ConvPhase &ph, const Ope
     j.chunk16 = j.pf_len16[0];  // slot size = largest chunk (tap (0,0): all four phases)
     j.oy_mul = j.ox_mul = 2; j.oy_off = j.ox_off = 0;
   }
-  // K-split between the two issuing warps (conv_tc.cu): one-row units whose accumulator needs <= 128 columns
-  {
-    const int cols = ph.rf_R ? ph.rf_R * ph.Npad : ph.Npad;
-    const bool ok = j.mt == 1 || ph.rf_R;
-    j.ksplit = (ok && cols <= 128 && (!ph.pf || ph.spc % 2 == 0) && !getenv("FAV_NO_KSPLIT")) ? 1 : 0;
-    if (!ph.rf_R && !ph.pf && (int)ph.steps.size() * ph.nrg * ph.nchg < 2) j.ksplit = 0;
-  }
+  j.ksplit = 0;
   if (ph.rf_R) {  // per-patch-row issue table (conv_tc.cu, row-fold loop)
     const int KH = j.rf_kh, R = j.rf_R, nblk = j.rf_nblk;
     if (j.rf_total_rows > kMaxRfRows) { set_error("conv %s: row-fold unit too tall", c.name.c_str()); return FAV_ERR_UNSUPPORTED; }

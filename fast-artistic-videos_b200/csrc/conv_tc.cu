@@ -1,94 +1,53 @@
-// conv_tc.cu -- the hot kernel: implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05, sm_100a).
+// conv_tc.cu -- the hot kernel: implicit-GEMM convolution on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces the cuDNN / THNN SpatialConvolution + SpatialFullConvolution calls of the reference net
 // (fast_artistic_video/models_video.lua:80,93,102; fast_artistic_video_core.lua:48-55).
 //
-// GEMM view (per job):  D[128 pixels, Npad couts] += A[128 pixels, K] * B[Npad, K]^T,
+// GEMM view (per tile):  D[128 pixels, Npad couts] += A[128 pixels, K] * B[Npad, K]^T,
 //   K = taps x input channels, walked in K=16 steps (two 8-channel "units" per step).
 // Precision: the reference computes in fp32.  A single fp16/tf32 pass misses the 1e-3 parity bar
 // (measured 1.2e-3..2.7e-3, DESIGN.md §precision), so every operand is an fp16 pair x = hi + lo and each
-// K step issues three MMAs  hi*hi + lo*hi + hi*lo  (fp32 accumulation in TMEM): ~2^-21 relative error at
-// 1.5x the cost of one TF32 pass.
+// K step issues three MMAs  hi*hi + lo*hi + hi*lo  (fp32 accumulation): ~2^-21 relative error.
 //
 // Data movement: the input patch of a tile (all filter rows x a group of channel blocks x 128+halo pixels)
-// is fetched ONCE per tile by 1-D bulk async copies (cp.async.bulk -> SASS UBLKCP, completion on an
-// mbarrier).  Because the operand layout in HBM is already the canonical no-swizzle K-major core-matrix
-// layout (net_layout.cuh), every filter tap reuses the same shared-memory patch: the UMMA matrix descriptor
-// just starts 16 B * dx further.  Weights stream through a ring of pre-packed chunks.
+// is fetched ONCE per tile by 1-D bulk async copies (cp.async.bulk, completion on an mbarrier).  Because the
+// operand layout in HBM is already the canonical no-swizzle K-major core-matrix layout (net_layout.cuh), every
+// filter tap reuses the same shared-memory patch: the wgmma matrix descriptor just starts 16 B * dx further.
+// Weights stream through a ring of pre-packed chunks (or stay resident when the layer's weights fit).
 //
-// Warp roles (480 threads = 15 warps, 1 CTA / SM, persistent over work units):
-//   warps 0-3, 8-11  epilogue (TMEM lane quarter = warp % 4; the two groups split column chunks / output rows):
-//                    tcgen05.ld TMEM -> registers -> +bias -> float4 stores + fused InstanceNorm statistics
-//                    (or x-fold reduction + tanh/deprocess for the last layer)
-//   warp  4          A producer (bulk copies of the patch, all lanes issue)
-//   warp  5          B producer (bulk copies of weight chunks; resident when the layer's weights fit)
-//   warps 6, 7       MMA issuers (6 also allocates TMEM): one accumulator row each for two-row units, alternate K steps
-//                    (K-split, accumulators at columns +0 / +128, summed by the epilogue) for one-row units
-//   warps 12-14      extra patch producers of norm-on-load jobs (with warp 4 and 8-11: raw fp32 -> InstanceNorm + ReLU ->
-//                    fp16 hi/lo staged for the MMA, replacing a separate in_apply pass)
-// Plans per layer family (conv_plan.hpp): generic, stride-2 parity split, tap pairing (Cin = 8), x-fold, row-fold, phase-fold.
-// Pipelines: A stages and weight slots (ring, or resident for small layers) with full/empty mbarriers; TMEM accumulator
-// double-buffered so the epilogue of unit i overlaps the MMAs of unit i+1.
+// Warp roles (persistent CTAs, 1 per SM):
+//   warps 0-7   two consumer warpgroups: warpgroup w issues the wgmmas of tile pixels [64w, 64w + 64) (M = 64, N = Npad,
+//               accumulators in registers) and runs their epilogue: +bias -> stores + fused InstanceNorm statistics
+//               (or x-fold reduction + tanh/deprocess for the last layer)
+//   warp  8     B producer (bulk copies of weight chunks)
+//   warp  9     A producer (bulk copies of the patch, all lanes issue)
+//   warps 9-12  norm-on-load jobs: patch producers (raw fp32 -> InstanceNorm + ReLU -> fp16 hi/lo staged for the MMA,
+//               replacing a separate in_apply pass)
+// Plans per layer family (conv_plan.hpp): generic, stride-2 parity split, tap pairing (Cin = 8), x-fold.
+// Pipelines: A stages and weight slots with full/empty mbarriers; each consumer warpgroup releases a slot once its
+// wgmmas that read it have completed.
+#include <atomic>
+
 #include "conv.cuh"
 #include "tc_common.cuh"
+#include "wgmma_f16.cuh"
 
 namespace fav {
 
 constexpr int kMaxA = 4;  // patch stages
-constexpr int kMaxSpc = 8;  // K16 steps per weight chunk (conv_plan.hpp caps spc at this)
 constexpr int kMaxB = 16;  // weight slots (ring or resident)
-constexpr int kTmemCols = 512;  // 2 accumulator stages x 256 columns (two rows / two K-split halves x <= 128, or one x 256)
-constexpr int kThreads = 480;  // warps 0-3 + 8-11 epilogue (TMEM lane quarter = warp % 4), 4 A producer, 5 B producer, 6/7 MMA issuers,
-                                // 12..14 extra patch producers of norm-on-load jobs
-constexpr int kNlWarps = 8;     // warps 4, 8..11 (the second epilogue group turns producer), 12, 13, 14
+constexpr int kConsumerThreads = 256;  // warps 0-7
+constexpr int kBWarp = 8, kAWarp = 9;
+constexpr int kNlWarps = 4;            // norm-on-load producers: warps 9..12
+constexpr int kThreads = kConsumerThreads + 32 * (1 + kNlWarps);  // launched with 320 threads when nl == 0
 constexpr int kNlPx = 5;        // pixels in flight per lane (5 x 32 >= the 130-pixel patch row)
 constexpr int kNlMaxC = 256;
 constexpr int kExchPitch = 33;  // fp32 words per pixel in the x-fold exchange buffer (odd: conflict-free)
+constexpr uint64_t kDescHi = (uint64_t)8u << 32;  // matrix descriptor: SBO = 8 x 16 B between 8-row core-matrix groups
 
 struct __align__(16) TcShared {
-  uint64_t a_full[kMaxA], a_empty[kMaxA], b_full[kMaxB], b_empty[kMaxB], t_full[2], t_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad_;
+  uint64_t a_full[kMaxA], a_empty[kMaxA], b_full[kMaxB], b_empty[kMaxB];
 };
-
-// accumulator columns [taddr, taddr+16) as floats; K-split jobs add the second issuing warp's partial sums (+128 columns)
-__device__ __forceinline__ void tmem_ld16_acc(uint32_t taddr, bool ksplit, float (&v)[16]) {
-  uint32_t r[16];
-  if (ksplit) {
-    uint32_t q[16];
-    tmem_ld16x2(taddr, taddr + 128u, r, q);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]) + __uint_as_float(q[i]);
-  } else {
-    tmem_ld16(taddr, r);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-  }
-}
-
-// sum over the 32 lanes of each of 16 per-lane values; lane L returns the total of value index (L >> 1)
-__device__ __forceinline__ float warp_reduce16(const float (&v)[16], int lane) {
-  float a[8], b[4], c[2];
-  const bool u16 = lane & 16, u8 = lane & 8, u4 = lane & 4, u2 = lane & 2;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    float send = u16 ? v[i] : v[i + 8], keep = u16 ? v[i + 8] : v[i];
-    a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float send = u8 ? a[i] : a[i + 4], keep = u8 ? a[i + 4] : a[i];
-    b[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-  }
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    float send = u4 ? b[i] : b[i + 2], keep = u4 ? b[i + 2] : b[i];
-    c[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-  }
-  float send = u2 ? c[0] : c[1], keep = u2 ? c[1] : c[0];
-  float d = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  return d + __shfl_xor_sync(0xffffffffu, d, 1);
-}
 
 __device__ __forceinline__ float tc_final_value(float v, int k, int mode, float tanh_c) {
   float t = tanhf(v) * tanh_c;  // nn.Tanh -> nn.MulConstant(150) (models_video.lua:135-136)
@@ -100,15 +59,157 @@ __device__ __forceinline__ float tc_final_value(float v, int k, int mode, float 
 }
 
 // ---- optional per-CTA timeline (job.trace != null; tools/trace_conv.py) ------------------------------------------------
-// word 0: globaltimer at entry (ns), 1: clock64 at entry, 2: clock64 after setup (barriers, TMEM), 3: clock64 at exit,
-// 4: units of this CTA; then per unit u < kTraceUnits at 8 + 8u: +0 MMA warp 6: accumulator stage free (unit start),
-// +1 first patch stage landed, +2 all MMAs issued, +3 cycles spent waiting for patch stages, +4 ... for weight chunks,
-// +5 epilogue warp 0: accumulator complete, +6 epilogue of the unit done.  clock64 values are per-SM cycle counters.
+// word 0: globaltimer at entry (ns), 1: clock64 at entry, 2: clock64 after setup, 3: clock64 at exit, 4: units of this CTA.
 __device__ __forceinline__ void trace_put(const ConvJob &job, int word, long long v) {
   if (job.trace) job.trace[(size_t)blockIdx.x * kTraceWords + word] = (unsigned long long)v;
 }
-__device__ __forceinline__ long long trace_clock(const ConvJob &job) { return job.trace ? clock64() : 0; }
 
+// consumer warpgroup: MMAs of one 64-pixel half of every tile of this CTA, then its epilogue
+template <int NT>
+__device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, uint8_t *b_base, TcShared *sh, float *exch) {
+  constexpr int NJ = NT / 8;
+  const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t a_stage_bytes = (uint32_t)job.stage16 * 16u, chunk_bytes = (uint32_t)job.chunk16 * 16u;
+  const uint32_t nstages = (uint32_t)job.a_stages, nslots = (uint32_t)job.b_slots;
+  const int ngroups = job.ngroups, nchunks = job.nchunks, spc = job.spc;
+  const uint32_t b_step16 = 2u * (uint32_t)NT, b_lo16 = (uint32_t)spc * b_step16, a_stage16 = (uint32_t)job.stage16;
+  const uint32_t *steps32 = reinterpret_cast<const uint32_t *>(job.steps);
+  // this thread's accumulator rows (pixels of the tile) and column pairs
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), q2 = 2 * (lane & 3);
+  float *slot = exch + 256;  // fused statistics: per-warp partial sums [8 warps][2][128], fixed summation order
+  float acc[NT / 2];
+  uint32_t sa = 0, aph = 0, sb = 0, bph = 0, tl = 0;
+  for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x, ++tl) {
+    if (job.b_resident) sb = 0;
+    uint32_t scale = 0;
+    for (int g = 0; g < ngroups; ++g) {
+      mbar_wait(&sh->a_full[sa], aph);
+      // A descriptor start: pixel r of the patch is at +16 B * r, this warpgroup's rows begin 64 pixels in
+      const uint32_t a_hi16 = (smem_u32(a_base + sa * 2 * a_stage_bytes) >> 4) + (uint32_t)wg * 64u, a_lo16 = a_hi16 + a_stage16;
+      uint32_t sidx = 0;
+      for (int c = 0; c < nchunks; ++c) {
+        if (!job.b_resident || tl == 0) mbar_wait(&sh->b_full[sb], job.b_resident ? 0u : bph);
+        const uint32_t bh = (smem_u32(b_base + sb * chunk_bytes) >> 4) | ((uint32_t)NT << 16);  // LBO = Npad rows
+        wgmma_fence();
+        uint32_t bs = bh;
+        for (int st = 0; st < spc; ++st, bs += b_step16) {
+          const uint32_t dls = steps32[sidx + st];  // a_off16 | lbo16 << 16 (conv.cuh KStep)
+          const uint64_t ad_hi = kDescHi | (a_hi16 + dls), ad_lo = kDescHi | (a_lo16 + dls);
+          const uint64_t bd_hi = kDescHi | bs, bd_lo = kDescHi | (bs + b_lo16);
+          Wgmma<NT>::mma(acc, ad_hi, bd_hi, scale);
+          Wgmma<NT>::mma(acc, ad_lo, bd_hi, 1u);
+          Wgmma<NT>::mma(acc, ad_hi, bd_lo, 1u);
+          scale = 1;
+        }
+        wgmma_commit();
+        wgmma_wait<0>();  // the slot's operands are consumed: release it
+        if (!job.b_resident && wt == 0) mbar_arrive(&sh->b_empty[sb]);
+        sidx += (uint32_t)spc;
+        if (++sb == nslots) { sb = 0; bph ^= 1; }
+      }
+      if (wt == 0) mbar_arrive(&sh->a_empty[sa]);
+      if (++sa == nstages) { sa = 0; aph ^= 1; }
+    }
+    if (job.dbg & 8) continue;
+
+    // ===== epilogue from registers: acc[4i + 2h + e] = (pixel r0 + 8h, column 8i + q2 + e) =====
+    const int yu = tile / job.tiles_x, x0 = (tile - yu * job.tiles_x) * job.tile_dx;
+    const int y = yu, yo = y * job.oy_mul + job.oy_off;
+    if (job.xfold_kw) {
+      // partial sums Q[pixel][kx*Cout + co] -> shared memory, then out[x][co] = sum_kx Q[x + kx][kx*Cout + co]
+      const int ncol = job.xfold_kw * job.Cout;
+#pragma unroll
+      for (int i = 0; i < NJ; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * i + q2 + e;
+            if (col < ncol) exch[(r0 + 8 * h) * kExchPitch + col] = acc[4 * i + 2 * h + e];
+          }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      const int px = threadIdx.x, x = x0 + px;
+      if (px < job.tile_dx && x < job.Wo && y < job.Ho && !(job.dbg & 1)) {
+        const int xo = x * job.ox_mul + job.ox_off;
+        const float *qv = exch + px * kExchPitch;
+        const int64_t plane = (int64_t)job.Ho * job.Wo, o = (int64_t)yo * job.Wo + xo;
+        for (int k = 0; k < job.Cout; ++k) {
+          float sum = __ldg(job.bias + k);
+          for (int kx = 0; kx < job.xfold_kw; ++kx) sum += qv[kx * (kExchPitch + job.Cout) + k];
+          job.out3[(job.final_mode == 2 ? 2 - k : k) * plane + o] = tc_final_value(sum, k, job.final_mode, job.tanh_c);
+        }
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");  // exch is rewritten by the next tile
+      continue;
+    }
+    bool valid[2];
+    int xo[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int x = x0 + r0 + 8 * h;
+      valid[h] = x < job.Wo && y < job.Ho && !(job.dbg & 1);
+      xo[h] = x * job.ox_mul + job.ox_off;
+    }
+    if (job.final_mode) {
+      // Cout <= 3 output channels sit in column group 0
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int k = q2 + e;
+          if (k < 3 && k < job.Cout && valid[h])
+            job.out3[((int64_t)(job.final_mode == 2 ? 2 - k : k) * job.Ho + yo) * job.Wo + xo[h]] =
+                tc_final_value(acc[2 * h + e] + __ldg(job.bias + k), k, job.final_mode, job.tanh_c);
+        }
+      continue;
+    }
+    const bool stats = job.stats && !(job.dbg & 64);
+#pragma unroll
+    for (int i = 0; i < NJ; ++i) {
+      const int c = 8 * i + q2;
+      const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c));
+      float v[4];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        v[2 * h] = acc[4 * i + 2 * h] + b.x;
+        v[2 * h + 1] = acc[4 * i + 2 * h + 1] + b.y;
+        // raw layout [Ho][Cq][Wp][4]: channels c, c + 1 of one pixel are 8 contiguous bytes
+        if (valid[h] && c < job.Cout)
+          *reinterpret_cast<float2 *>(job.raw + (((int64_t)yo * job.raw_Cq + (c >> 2)) * job.raw_Wp + xo[h]) * 4 + (c & 3)) =
+              make_float2(v[2 * h], v[2 * h + 1]);
+        if (!valid[h]) v[2 * h] = v[2 * h + 1] = 0.f;
+      }
+      if (stats) {
+        // per-channel sums over the warp's 16 pixels: reduce over the 8 lanes that share lane % 4
+        float s0 = v[0] + v[2], s1 = v[1] + v[3], t0 = v[0] * v[0] + v[2] * v[2], t1 = v[1] * v[1] + v[3] * v[3];
+#pragma unroll
+        for (int m = 4; m < 32; m <<= 1) {
+          s0 += __shfl_xor_sync(0xffffffffu, s0, m); s1 += __shfl_xor_sync(0xffffffffu, s1, m);
+          t0 += __shfl_xor_sync(0xffffffffu, t0, m); t1 += __shfl_xor_sync(0xffffffffu, t1, m);
+        }
+        if (lane < 4) {  // one writer per (warp, channel): deterministic
+          float *sl = slot + warp * 256;
+          sl[c] += s0; sl[c + 1] += s1; sl[128 + c] += t0; sl[128 + c + 1] += t1;
+        }
+      }
+    }
+  }
+  if (job.stats) {
+    // 8 warps' partial sums added in a FIXED order (deterministic per CTA: the tile -> CTA assignment is static), then one
+    // double atomic per channel and quantity per CTA
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    const int ch = threadIdx.x;
+    if (ch < job.Cout) {
+      float ssum = 0.f, qsum = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) { ssum += slot[w * 256 + ch]; qsum += slot[w * 256 + 128 + ch]; }
+      atomicAdd(job.stats + ch, (double)ssum);
+      atomicAdd(job.stats + job.Cout + ch, (double)qsum);
+    }
+  }
+}
+
+template <int NT>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ ConvJob job) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t a_stage_bytes = (uint32_t)job.stage16 * 16u;  // one of hi / lo
@@ -118,6 +219,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   uint8_t *b_base = a_base + nstages * 2 * a_stage_bytes;   // slot s: [hi steps][lo steps]
   const uint32_t nslots = (uint32_t)job.b_slots;
   TcShared *sh = reinterpret_cast<TcShared *>(b_base + nslots * chunk_bytes);
+  float *exch = reinterpret_cast<float *>(sh + 1);  // x-fold exchange buffer [128][kExchPitch] / statistics slots
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (job.trace && threadIdx.x == 0) {
@@ -126,59 +228,43 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     trace_put(job, 0, (long long)gt);
     trace_put(job, 1, clock64());
   }
-
-  // Two-row units (mt = 2) are issued by TWO warps, one accumulator row each: a single warp sustains only ~1 UTCHMMA per
-  // 80-100 cycles on this loop (tools/mma_bench3.cu), two warps reach the 64-cycle tensor-pipe floor.
-  // Other units may be K-split (job.ksplit): the two warps take alternate K steps (patch rows for row-fold) into two
-  // accumulators (columns +0 / +128) that the epilogue adds.
-  const bool dual_rows = job.mt == 2 && !job.rf_R && !job.pf, ksplit = job.ksplit != 0;
-  const bool dual = dual_rows || ksplit;
-  const uint32_t nissue = dual ? 2u : 1u;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kMaxA; ++i) { mbar_init(&sh->a_full[i], job.nl == 1 ? kNlWarps : (job.nl == 2 ? 4 : 1)); mbar_init(&sh->a_empty[i], nissue); }
-    for (int i = 0; i < kMaxB; ++i) { mbar_init(&sh->b_full[i], 1); mbar_init(&sh->b_empty[i], nissue); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&sh->t_full[i], nissue); mbar_init(&sh->t_empty[i], job.nl == 1 ? 128 : 256); }
+    for (int i = 0; i < kMaxA; ++i) { mbar_init(&sh->a_full[i], job.nl ? kNlWarps : 1); mbar_init(&sh->a_empty[i], 2); }
+    for (int i = 0; i < kMaxB; ++i) { mbar_init(&sh->b_full[i], 1); mbar_init(&sh->b_empty[i], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 6) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sh->tmem_base)),
-                 "r"((uint32_t)kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
+  if (job.stats && !job.xfold_kw)
+    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) exch[256 + i] = 0.f;
   // norm-on-load: mean / gamma*rstd / beta per input channel from the producer conv's fused statistics (same arithmetic
   // as in_apply_kernel: biased variance, eps inside the sqrt, InstanceNormalization.lua:39-50)
-  float *nl_tab = reinterpret_cast<float *>(sh + 1) + (256 + 8 * 2 * 128);
-  if (job.nl && (int)threadIdx.x < job.nl_C) {
-    const int c = threadIdx.x;
-    in_finalize(job.nl_sums[c], job.nl_sums[job.nl_C + c], job.nl_inv_count, job.nl_eps, job.nl_gamma[c], nl_tab[c], nl_tab[kNlMaxC + c]);
-    nl_tab[2 * kNlMaxC + c] = job.nl_beta[c];
-  }
-  tc_fence_before();
+  float *nl_tab = exch + (256 + 8 * 2 * 128);
+  if (job.nl)
+    for (int c = threadIdx.x; c < job.nl_C; c += blockDim.x) {
+      in_finalize(job.nl_sums[c], job.nl_sums[job.nl_C + c], job.nl_inv_count, job.nl_eps, job.nl_gamma[c], nl_tab[c], nl_tab[kNlMaxC + c]);
+      nl_tab[2 * kNlMaxC + c] = job.nl_beta[c];
+    }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sh->tmem_base;
-  if (threadIdx.x == 0) trace_put(job, 2, trace_clock(job));
+  if (threadIdx.x == 0 && job.trace) trace_put(job, 2, clock64());
 
-  const int ngroups = job.ngroups, nchunks = job.nchunks, spc = job.spc, Npad = job.Npad;
+  const int ngroups = job.ngroups, nchunks = job.nchunks;
 
-  if (job.nl && (warp == 4 || (warp >= 12 && warp <= 14) || (job.nl == 1 && warp >= 8 && warp <= 11))) {
+  if (warp < 8) {
+    tc_consume<NT>(job, a_base, b_base, sh, exch);
+  } else if (job.nl && warp >= kAWarp) {
     // ===== norm-on-load patch producers: raw fp32 -> InstanceNorm (+ReLU) -> fp16 hi/lo -> MMA-ready stage =====
     // A warp owns whole (patch row, channel block) slabs: lanes run along x (coalesced 512-byte loads), up to
     // kNlPx float4 pairs in flight per lane, no per-pixel index arithmetic.
-    // nl == 1: 8 producer warps (4, 8..14; one epilogue group); nl == 2: 4 producer warps (4, 12..14; two epilogue groups)
-    const int nlw = job.nl == 1 ? kNlWarps : 4;
-    const int pw = warp == 4 ? 0 : (job.nl == 1 ? warp - 7 : warp - 11);
+    const int pw = warp - kAWarp;
     const int pslab = job.pslab16, nslabs = job.nrows * job.CbG;
     uint32_t s = 0, ph = 0;
     for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) {
       const int yu = tile / job.tiles_x, x0 = (tile - yu * job.tiles_x) * job.tile_dx;
-      const int y = yu * job.mt;
+      const int y = yu;
       const int xb = job.seg_src16[0] + x0 - job.nl_padL;  // raw column of patch pixel 0
       for (int g = 0; g < ngroups; ++g) {
         mbar_wait(&sh->a_empty[s], ph ^ 1);
         uint8_t *stage = a_base + s * 2 * a_stage_bytes;
-        for (int rc = pw; rc < nslabs; rc += nlw) {
+        for (int rc = pw; rc < nslabs; rc += kNlWarps) {
           const int ri = rc / job.CbG, cbi = rc - ri * job.CbG;
           const int ry = job.row_mul * y + job.grp_row[g][ri] - job.nl_padT, cb = job.grp_cb0[g] + cbi;
           const bool row_ok = ry >= 0 && ry < job.nl_H;
@@ -216,24 +302,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
               }
               uint32_t h[4], l[4];  // same values as split_store8 (net_kernels.cu), packed two per conversion
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                split_pair(v[2 * i], v[2 * i + 1], h[i], l[i]);
-              }
+              for (int i = 0; i < 4; ++i) split_pair(v[2 * i], v[2 * i + 1], h[i], l[i]);
               *reinterpret_cast<uint4 *>(drow + (uint32_t)p * 16u) = make_uint4(h[0], h[1], h[2], h[3]);
               *reinterpret_cast<uint4 *>(drow + a_stage_bytes + (uint32_t)p * 16u) = make_uint4(l[0], l[1], l[2], l[3]);
             }
           }
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to tcgen05.mma
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to wgmma
         __syncwarp();
         if (lane == 0) mbar_arrive(&sh->a_full[s]);
         if (++s == nstages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 4) {
+  } else if (warp == kAWarp) {
     // ===== A producer: the input patch of each (tile, channel group): one bulk copy per (patch row, channel block, hi/lo),
-    // spread over the 32 lanes.  (Measured alternatives, all slower on B200 and removed: four producer warps sharing the
-    // copies, a single elected lane with warp-uniform operands, one 4-D cp.async.bulk.tensor per plane -- DESIGN.md 9.3.) =====
+    // spread over the 32 lanes =====
     const int per_row = job.CbG * job.nseg * 2;  // copies per patch row (x2: hi, lo)
     const int ncopies = job.nrows * per_row;
     uint32_t stage_tx = 0;
@@ -242,7 +325,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     uint32_t s = 0, ph = 0;
     for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) {
       const int yu = tile / job.tiles_x, x0 = (tile - yu * job.tiles_x) * job.tile_dx;
-      const int y = yu * job.mt;
+      const int y = yu;
       for (int g = 0; g < ngroups; ++g) {
         mbar_wait(&sh->a_empty[s], ph ^ 1);
         if (lane == 0) mbar_arrive_expect_tx(&sh->a_full[s], stage_tx);
@@ -263,28 +346,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         if (++s == nstages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 5) {
+  } else if (warp == kBWarp) {
     // ===== B producer: weight chunks =====
     if (lane == 0) {
       uint32_t s = 0, ph = 0;
-      if (job.rf_R) {  // row-fold: one resident chunk per K step, shared by every patch row
-        for (int c = 0; c < job.rf_steps; ++c) {
-          mbar_arrive_expect_tx(&sh->b_full[c], chunk_bytes);
-          bulk_g2s(b_base + c * chunk_bytes, job.b + (int64_t)c * job.chunk16, chunk_bytes, &sh->b_full[c]);
-        }
-      } else if (job.pf) {  // phase-fold: one chunk per (channel group, tap), sizes differ per tap
-        for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) {
-          if (job.b_resident && tile != (int)blockIdx.x) break;
-          for (int g = 0; g < ngroups; ++g)
-            for (int c = 0; c < 4; ++c) {
-              mbar_wait(&sh->b_empty[s], ph ^ 1);
-              const uint32_t cb = (job.dbg & 2) ? 16u : (uint32_t)job.pf_len16[c] * 16u;
-              mbar_arrive_expect_tx(&sh->b_full[s], cb);
-              bulk_g2s(b_base + s * chunk_bytes, job.b + (int64_t)g * job.pf_grp16 + job.pf_src16[c], cb, &sh->b_full[s]);
-              if (++s == nslots) { s = 0; ph ^= 1; }
-            }
-        }
-      } else
       for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) {
         if (job.b_resident && tile != (int)blockIdx.x) break;  // resident weights: one pass fills every slot
         for (int g = 0; g < ngroups; ++g)
@@ -298,388 +363,20 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
       }
     }
     __syncwarp();
-  } else if (warp == 6 || (warp == 7 && dual)) {
-    // ===== MMA issuer: the whole warp runs the (warp-uniform) control flow so that descriptors live in uniform
-    // registers and the UTCHMMAs issue back to back; one elected lane executes the tcgen05 instructions =====
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    // instruction descriptor: D=f32 (bits 4-5 = 1), A=B=f16 (0), K-major both, N>>3 at [17,23), M>>4 at [24,29)
-    const uint32_t idesc = (1u << 4) | ((uint32_t)(Npad >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
-    // Matrix descriptors (K-major, no swizzle).  High word is constant: SBO = 8 (128 B between 8-row groups) and
-    // descriptor version 1 (bit 46).  Low word = start address>>4 | LBO<<16.  A KStep table entry is exactly the
-    // 32-bit word (a_off16 | lbo16 << 16), so the A descriptor of a step is one add on the uniform datapath; the
-    // dependent chain in front of each UTCHMMA is kept to that single add (the uniform pipe is slow on long chains:
-    // ~250 cycles/step when the descriptors were rebuilt per step, measured with FAV_DBG ablations).
-    const uint32_t desc_hi = 8u | (1u << 14);
-    const uint32_t b_step16 = 2u * (uint32_t)Npad, b_lo16 = (uint32_t)spc * b_step16;
-    const uint32_t a_tile16 = (uint32_t)(job.CbG * job.pslab16);  // mt = 2: second output row = one patch row lower
-    const uint32_t a_stage16 = (uint32_t)job.stage16;
-    const uint32_t *steps32 = reinterpret_cast<const uint32_t *>(job.steps);
-    const uint32_t drow = dual ? (uint32_t)(warp - 6) : 0u;  // dual issue: this warp's accumulator row
-    // NOTE: no runtime integer division / modulo on this warp: ~150 cycles each on the issue path (measured with
-    // tools/mma_bench.cu); ring positions are wrap counters.
-    uint32_t sa = 0, aph = 0, tl = 0, sb = 0, bph = 0;
-    for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x, ++tl) {
-      const uint32_t as = tl & 1, tph = (tl >> 1) & 1;
-      mbar_wait(&sh->t_empty[as], tph ^ 1);
-      tc_fence_after();
-      const bool tr = job.trace && warp == 6 && lane == 0 && tl < (uint32_t)kTraceUnits;
-      long long tr_a = 0, tr_b = 0;
-      if (tr) trace_put(job, 8 + 8 * (int)tl, clock64());
-      const uint32_t d0 = tmem_base + as * 256u + drow * 128u;
-      if (job.rf_R) {
-        // ===== row-fold issue loop (conv.cuh): patch row iy feeds output rows r_min..r_max in ONE MMA per K step =====
-        const int KH = job.rf_kh, R = job.rf_R;
-        const uint32_t nblk = (uint32_t)job.rf_nblk, NR = (uint32_t)KH * nblk;  // weight rows per k-half
-        const uint32_t idesc_base = (1u << 4) | ((uint32_t)(kTileM >> 4) << 24);
-        if (tl == 0)
-          for (int c = 0; c < job.rf_steps; ++c) mbar_wait(&sh->b_full[c], 0);
-        tc_fence_after();
-        const uint32_t b16 = smem_u32(b_base) >> 4;
-        for (int g = 0; g < ngroups; ++g) {
-          mbar_wait(&sh->a_full[sa], aph);
-          tc_fence_after();
-          const uint32_t a_hi16 = smem_u32(a_base + sa * 2 * a_stage_bytes) >> 4, a_lo16 = a_hi16 + a_stage16;
-          if (leader) {
-            for (int ri = 0; ri < job.nrows; ++ri) {
-              const int iy = g * job.nrows + ri;
-              if (ksplit && (uint32_t)(iy & 1) != drow) continue;      // K-split: this warp owns patch rows of its parity
-              // host-computed per-row table (conv_plan.hpp): columns, weight slice and descriptors of the rows fed
-              const uint32_t dcol = d0 + job.rf_dcol[iy], boff = job.rf_boff[iy];
-              const uint32_t idn_all = job.rf_idn_all[iy], idn_acc = job.rf_idn_acc[iy], idn_new = job.rf_idn_new[iy];
-              const uint32_t off_new = job.rf_off_new[iy];
-              const uint32_t arow = (uint32_t)ri * (uint32_t)job.rf_row16;
-              for (int st = 0; st < job.rf_steps; ++st) {
-                const uint32_t dls = steps32[st];
-                const uint64_t ad_hi = ((uint64_t)desc_hi << 32) | (a_hi16 + arow + dls), ad_lo = ((uint64_t)desc_hi << 32) | (a_lo16 + arow + dls);
-                // weight chunk st: [hi: 2 k-halves x NR rows][lo: ...]; LBO = NR rows
-                const uint32_t bq = (b16 + (uint32_t)st * (uint32_t)job.chunk16 + boff) | (NR << 16);
-                const uint64_t bd_hi = ((uint64_t)desc_hi << 32) | bq, bd_lo = ((uint64_t)desc_hi << 32) | (bq + 2u * NR);
-                if (st == 0 && idn_new) {
-                  if (idn_acc) {  // rows that already hold partial sums
-                    tc_mma_f16(dcol, ad_hi, bd_hi, idn_acc, 1);
-                    tc_mma_f16(dcol, ad_lo, bd_hi, idn_acc, 1);
-                    tc_mma_f16(dcol, ad_hi, bd_lo, idn_acc, 1);
-                  }
-                  // rows this warp touches for the first time (r = iy; K-split: r = iy - 1 as well): overwrite
-                  tc_mma_f16(dcol + off_new, ad_hi, bd_hi + off_new, idn_new, 0);
-                  tc_mma_f16(dcol + off_new, ad_lo, bd_hi + off_new, idn_new, 1);
-                  tc_mma_f16(dcol + off_new, ad_hi, bd_lo + off_new, idn_new, 1);
-                } else {
-                  tc_mma_f16(dcol, ad_hi, bd_hi, idn_all, 1);
-                  tc_mma_f16(dcol, ad_lo, bd_hi, idn_all, 1);
-                  tc_mma_f16(dcol, ad_hi, bd_lo, idn_all, 1);
-                }
-              }
-            }
-            tc_commit(&sh->a_empty[sa]);
-          }
-          if (++sa == nstages) { sa = 0; aph ^= 1; }
-        }
-        if (leader) tc_commit(&sh->t_full[as]);
-        continue;
-      }
-      if (job.b_resident) sb = 0;
-      if (job.pf) {
-        // ===== phase-fold issue loop: chunk c = tap c; its MMAs write pf_n[c] columns starting at pf_col[c] =====
-        const uint32_t idesc_base = (1u << 4) | ((uint32_t)(kTileM >> 4) << 24);
-        uint32_t acc = 0;
-        for (int g = 0; g < ngroups; ++g) {
-          mbar_wait(&sh->a_full[sa], aph);
-          tc_fence_after();
-          const uint32_t a_hi16 = smem_u32(a_base + sa * 2 * a_stage_bytes) >> 4, a_lo16 = a_hi16 + a_stage16;
-          for (int c = 0; c < 4; ++c) {
-            if (!job.b_resident || tl == 0) {
-              mbar_wait(&sh->b_full[sb], job.b_resident ? 0u : bph);
-              tc_fence_after();
-            }
-            const uint32_t n = (uint32_t)job.pf_n[c], dcol = d0 + (uint32_t)job.pf_col[c];
-            const uint32_t idn = idesc_base | ((n >> 3) << 17);
-            const uint32_t bq = (smem_u32(b_base + sb * chunk_bytes) >> 4) | (n << 16);   // LBO = n rows
-            const uint32_t blo = (uint32_t)spc * 2u * n;                                     // lo image follows the hi image
-            if (leader) {
-              for (int j = 0; j < spc; ++j) {
-                if (ksplit && (uint32_t)(j & 1) != drow) continue;  // K-split (spc is even)
-                const uint32_t dls = steps32[c * spc + j];
-                const uint64_t ad_hi = ((uint64_t)desc_hi << 32) | (a_hi16 + dls), ad_lo = ((uint64_t)desc_hi << 32) | (a_lo16 + dls);
-                const uint32_t bs = bq + (uint32_t)j * 2u * n;
-                const uint64_t bd_hi = ((uint64_t)desc_hi << 32) | bs, bd_lo = ((uint64_t)desc_hi << 32) | (bs + blo);
-                tc_mma_f16(dcol, ad_hi, bd_hi, idn, acc);  // acc == 0 only for the very first step: tap (0,0) covers all columns
-                tc_mma_f16(dcol, ad_lo, bd_hi, idn, 1);
-                tc_mma_f16(dcol, ad_hi, bd_lo, idn, 1);
-                acc = 1;
-              }
-              if (!job.b_resident) tc_commit(&sh->b_empty[sb]);
-            }
-            acc = 1;
-            if (++sb == nslots) { sb = 0; bph ^= 1; }
-          }
-          if (leader) tc_commit(&sh->a_empty[sa]);
-          if (++sa == nstages) { sa = 0; aph ^= 1; }
-        }
-        if (leader) tc_commit(&sh->t_full[as]);
-        continue;
-      }
-      // ===== generic issue loop.  The issuing warps are INSTRUCTION bound on the narrow layers (ncu source counters, d64: the
-      // two warps were busy in their own code all the time -- ~570 instructions per weight chunk in an unrolled, predicated
-      // step ladder, i-cache misses -- while the tensor pipe was 25 % active), so this is the leanest form: per chunk one
-      // divergent region holding a plain loop over the K steps, ~12 instructions per step around the three UTCHMMAs.
-      uint32_t acc = 0, sc = 0;  // acc: this warp's accumulator holds a partial sum; sc: K-step counter of the unit (K-split parity)
-      for (int g = 0; g < ngroups; ++g) {
-        long long tw = tr ? clock64() : 0;
-        mbar_wait(&sh->a_full[sa], aph);
-        tc_fence_after();
-        if (tr) { const long long now = clock64(); tr_a += now - tw; if (g == 0) trace_put(job, 8 + 8 * (int)tl + 1, now); }
-        const uint32_t a_hi16 = (smem_u32(a_base + sa * 2 * a_stage_bytes) >> 4) + (dual_rows ? drow * a_tile16 : 0u), a_lo16 = a_hi16 + a_stage16;
-        uint32_t sidx = 0;
-        for (int c = 0; c < nchunks; ++c) {
-          // ring: slot sb, phase bph.  resident: slot = chunk index, filled once (parity 0 stays satisfied afterwards)
-          if (!job.b_resident || tl == 0) {  // resident weights are complete after the first tile
-            const long long tw2 = tr ? clock64() : 0;
-            mbar_wait(&sh->b_full[sb], job.b_resident ? 0u : bph);
-            tc_fence_after();
-            if (tr) tr_b += clock64() - tw2;
-          }
-          const uint32_t bh = (smem_u32(b_base + sb * chunk_bytes) >> 4) | ((uint32_t)Npad << 16);  // LBO = Npad * 16 B
-          if (leader) {
-            uint32_t bs = bh;
-            for (uint32_t st = 0; st < (uint32_t)spc; ++st, bs += b_step16) {
-              if (ksplit && ((sc + st) & 1u) != drow) continue;  // K-split: alternate steps, one accumulator per warp
-              const uint32_t dls = steps32[sidx + st];
-              const uint64_t ad_hi = ((uint64_t)desc_hi << 32) | (a_hi16 + dls), ad_lo = ((uint64_t)desc_hi << 32) | (a_lo16 + dls);
-              const uint64_t bd_hi = ((uint64_t)desc_hi << 32) | bs, bd_lo = ((uint64_t)desc_hi << 32) | (bs + b_lo16);
-              tc_mma_f16(d0, ad_hi, bd_hi, idesc, acc);
-              tc_mma_f16(d0, ad_lo, bd_hi, idesc, 1);
-              tc_mma_f16(d0, ad_hi, bd_lo, idesc, 1);
-              acc = 1;
-            }
-            if (!job.b_resident) tc_commit(&sh->b_empty[sb]);  // frees the weight slot when the MMAs retire
-          }
-          sidx += (uint32_t)spc;
-          sc += (uint32_t)spc;
-          if (++sb == nslots) { sb = 0; bph ^= 1; }
-        }
-        if (leader) tc_commit(&sh->a_empty[sa]);  // frees the patch stage
-        if (++sa == nstages) { sa = 0; aph ^= 1; }
-      }
-      if (leader) tc_commit(&sh->t_full[as]);  // accumulator complete -> epilogue
-      if (tr) { trace_put(job, 8 + 8 * (int)tl + 2, clock64()); trace_put(job, 8 + 8 * (int)tl + 3, tr_a); trace_put(job, 8 + 8 * (int)tl + 4, tr_b); }
-    }
-    __syncwarp();
-  } else if (warp < 4 || (warp >= 8 && warp < 12 && job.nl != 1)) {
-    // ===== epilogue warps 0..3 (group 0) and 8..11 (group 1): TMEM lane = pixel; the two groups split the columns =====
-    uint32_t tl = 0;
-    const int wq = warp & 3, eg = warp >> 3;
-    const int neg = job.nl == 1 ? 1 : 2;  // norm-on-load (8-producer mode): the second group works as patch producers
-    const int px = wq * 32 + lane;
-    const int nj = (Npad + 15) >> 4;
-    const bool ks = job.ksplit != 0;
-    float *exch = reinterpret_cast<float *>(sh + 1);  // x-fold exchange buffer [128][kExchPitch] / stats [2][128]
-    float acc_s[8], acc_q[8];  // fused InstanceNorm statistics: this lane's channel (16*j + lane/2), all tiles
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc_s[j] = acc_q[j] = 0.f;
-
-    for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x, ++tl) {
-      const int yu = tile / job.tiles_x, x = (tile - yu * job.tiles_x) * job.tile_dx + px;
-      const uint32_t as = tl & 1, tph = (tl >> 1) & 1;
-      mbar_wait(&sh->t_full[as], tph);
-      tc_fence_after();
-      const bool etr = job.trace && threadIdx.x == 0 && tl < (uint32_t)kTraceUnits;
-      if (etr) trace_put(job, 8 + 8 * (int)tl + 5, clock64());
-      if (job.dbg & 8) { tc_fence_before(); mbar_arrive(&sh->t_empty[as]); continue; }
-      if (job.pf) {
-        // 4 phase blocks of pf_cout columns: block k -> output pixel (2y + a, 2x + b), (a,b) = (0,0),(0,1),(1,1),(1,0).
-        // Epilogue group eg owns output row a = eg; a thread stores the b = 0 / b = 1 pixels of one channel quad as 32
-        // contiguous bytes.
-        const int yi = yu;  // mt == 1
-        const bool valid = x < job.Wo && yi < job.Ho && !(job.dbg & 1);
-        const uint32_t taddr0 = tmem_base + ((uint32_t)(wq * 32) << 16) + as * 256u;
-        const int C = job.pf_cout;
-        const int a = eg, yo = 2 * yi + a;
-        const uint32_t col_b0 = (uint32_t)((a ? 3 : 0) * C), col_b1 = (uint32_t)((a ? 2 : 1) * C);
-#pragma unroll
-        for (int jc = 0; jc < 4; ++jc) {
-          const int c0 = jc * 16;
-          if (c0 >= C) break;
-          uint32_t r0[16], r1[16];
-          tmem_ld16x2(taddr0 + col_b0 + (uint32_t)c0, taddr0 + col_b1 + (uint32_t)c0, r0, r1);
-          float v0[16], v1[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) { v0[i] = __uint_as_float(r0[i]); v1[i] = __uint_as_float(r1[i]); }
-          if (ks) {  // second issuing warp's partial sums
-            tmem_ld16x2(taddr0 + 128u + col_b0 + (uint32_t)c0, taddr0 + 128u + col_b1 + (uint32_t)c0, r0, r1);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) { v0[i] += __uint_as_float(r0[i]); v1[i] += __uint_as_float(r1[i]); }
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 bq4 = __ldg(reinterpret_cast<const float4 *>(job.bias + c0) + q);
-            v0[4 * q] += bq4.x; v0[4 * q + 1] += bq4.y; v0[4 * q + 2] += bq4.z; v0[4 * q + 3] += bq4.w;
-            v1[4 * q] += bq4.x; v1[4 * q + 1] += bq4.y; v1[4 * q + 2] += bq4.z; v1[4 * q + 3] += bq4.w;
-          }
-          if (valid) {
-            float4 *rp = reinterpret_cast<float4 *>(job.raw) + (((int64_t)yo * job.raw_Cq + (c0 >> 2)) * job.raw_Wp + 2 * x);
-#pragma unroll
-            for (int q = 0; q < 4; ++q)  // ONE 256-bit store per channel quad: whole 32-byte sectors (two float4 stores wrote each sector twice)
-              asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(rp + (int64_t)q * job.raw_Wp), "f"(v0[4 * q]),
-                           "f"(v0[4 * q + 1]), "f"(v0[4 * q + 2]), "f"(v0[4 * q + 3]), "f"(v1[4 * q]), "f"(v1[4 * q + 1]),
-                           "f"(v1[4 * q + 2]), "f"(v1[4 * q + 3])
-                           : "memory");
-          }
-          if (job.stats && !(job.dbg & 64)) {
-            float sv[16], sq[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float e0 = valid ? v0[i] : 0.f, e1 = valid ? v1[i] : 0.f;
-              sv[i] = e0 + e1; sq[i] = e0 * e0 + e1 * e1;
-            }
-            acc_s[jc] += warp_reduce16(sv, lane);
-            acc_q[jc] += warp_reduce16(sq, lane);
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(&sh->t_empty[as]);
-        continue;
-      }
-      for (int t = 0; t < job.mt; ++t) {
-      const int y = yu * job.mt + t;
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + as * 256u +
-                             (uint32_t)t * (job.rf_R ? (uint32_t)job.rf_nblk : 128u);
-      const int yo = y * job.oy_mul + job.oy_off, xo = x * job.ox_mul + job.ox_off;
-      const bool valid = x < job.Wo && y < job.Ho && !(job.dbg & 1);
-      if (job.xfold_kw) {
-        // partial sums Q[pixel][kx*Cout + co] -> shared memory, then out[x][co] = sum_kx Q[x + kx][kx*Cout + co].
-        // Epilogue group eg owns the output rows t = eg (mod 2) of the unit: its own exchange buffer and named barrier.
-        const int last_t = ((job.mt - 1 - eg) & ~1) + eg;  // last row of this group (< 0: none)
-        if (t == 0 && last_t < 0) {
-          tc_fence_before();
-          mbar_arrive(&sh->t_empty[as]);
-        }
-        if ((t & 1) != eg) continue;
-        float *ex = exch + eg * (kTileM * kExchPitch);
-        for (int c0 = 0; c0 < Npad; c0 += 16) {
-          float r[16];
-          tmem_ld16_acc(taddr + (uint32_t)c0, ks, r);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) ex[px * kExchPitch + c0 + i] = r[i];
-        }
-        if (t == last_t) {
-          tc_fence_before();
-          mbar_arrive(&sh->t_empty[as]);  // TMEM stage drained: the next tile's MMAs may start
-        }
-        if (eg) asm volatile("bar.sync 2, 128;" ::: "memory"); else asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (px < job.tile_dx && valid) {
-          const float *q = ex + px * kExchPitch;
-          if (job.xfold_kw == 9 && job.Cout == 3) {
-            float s0 = __ldg(job.bias), s1 = __ldg(job.bias + 1), s2 = __ldg(job.bias + 2);
-#pragma unroll
-            for (int kx = 0; kx < 9; ++kx) {
-              const float *e = q + kx * (kExchPitch + 3);
-              s0 += e[0]; s1 += e[1]; s2 += e[2];
-            }
-            const int64_t plane = (int64_t)job.Ho * job.Wo, o = (int64_t)yo * job.Wo + xo;
-            const bool flip = job.final_mode == 2;
-            job.out3[(flip ? 2 : 0) * plane + o] = tc_final_value(s0, 0, job.final_mode, job.tanh_c);
-            job.out3[plane + o] = tc_final_value(s1, 1, job.final_mode, job.tanh_c);
-            job.out3[(flip ? 0 : 2) * plane + o] = tc_final_value(s2, 2, job.final_mode, job.tanh_c);
-          } else {
-            for (int k = 0; k < job.Cout; ++k) {
-              float sum = __ldg(job.bias + k);
-              for (int kx = 0; kx < job.xfold_kw; ++kx) sum += q[kx * (kExchPitch + job.Cout) + k];
-              job.out3[((int64_t)(job.final_mode == 2 ? 2 - k : k) * job.Ho + yo) * job.Wo + xo] =
-                  tc_final_value(sum, k, job.final_mode, job.tanh_c);
-            }
-          }
-        }
-        if (eg) asm volatile("bar.sync 2, 128;" ::: "memory"); else asm volatile("bar.sync 1, 128;" ::: "memory");  // ex is rewritten
-        continue;  // next output row of the unit
-      }
-#pragma unroll
-      for (int jc = 0; jc < 8; ++jc) {
-        const int c0 = jc * 16;
-        if (c0 >= Npad) break;
-        if (neg == 2 && (nj >= 2 ? ((jc + t) & 1) : (t & 1)) != eg) continue;  // work split between the two epilogue groups
-        float v[16];
-        tmem_ld16_acc(taddr + (uint32_t)c0, ks, v);
-        if (job.final_mode == 0) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 bq = __ldg(reinterpret_cast<const float4 *>(job.bias + c0) + q);
-            v[4 * q] += bq.x; v[4 * q + 1] += bq.y; v[4 * q + 2] += bq.z; v[4 * q + 3] += bq.w;
-          }
-          if (valid) {
-            float4 *rp = reinterpret_cast<float4 *>(job.raw) + (((int64_t)yo * job.raw_Cq + (c0 >> 2)) * job.raw_Wp + xo);
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              if (c0 + 4 * q < job.Cout) rp[(int64_t)q * job.raw_Wp] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          }
-          if (job.stats && !(job.dbg & 64)) {
-            // per-channel sums over the warp's 32 pixels: butterfly transpose-reduce, 16 shuffles per quantity;
-            // afterwards lane L holds channel c0 + (L >> 1)
-            float sq[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) { v[i] = valid ? v[i] : 0.f; sq[i] = v[i] * v[i]; }
-            acc_s[jc] += warp_reduce16(v, lane);
-            acc_q[jc] += warp_reduce16(sq, lane);
-          }
-        } else if (c0 == 0 && valid) {
-#pragma unroll
-          for (int k = 0; k < 3; ++k)
-            if (k < job.Cout)
-              job.out3[((int64_t)(job.final_mode == 2 ? 2 - k : k) * job.Ho + yo) * job.Wo + xo] =
-                  tc_final_value(v[k] + __ldg(job.bias + k), k, job.final_mode, job.tanh_c);
-        }
-      }
-      }  // t
-      if (!job.xfold_kw) {
-        tc_fence_before();
-        mbar_arrive(&sh->t_empty[as]);
-      }
-      if (etr) trace_put(job, 8 + 8 * (int)tl + 6, clock64());
-    }
-    if (job.stats) {
-      // 4 warps -> shared memory in per-warp slots, summed in a FIXED order (deterministic per CTA: the tile ->
-      // CTA assignment is static), then one double atomic per channel and quantity per CTA
-      float *slot = exch + 256;  // [8 warps][2][128]
-      const int ws = eg * 4 + wq;
-      if ((lane & 1) == 0) {
-#pragma unroll
-        for (int jc = 0; jc < 8; ++jc)
-          if (jc * 16 < (job.pf ? job.pf_cout : Npad)) {
-            slot[(ws * 2 + 0) * 128 + jc * 16 + (lane >> 1)] = acc_s[jc];
-            slot[(ws * 2 + 1) * 128 + jc * 16 + (lane >> 1)] = acc_q[jc];
-          }
-      }
-      if (neg == 2) asm volatile("bar.sync 1, 256;" ::: "memory"); else asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (eg == 0 && px < job.Cout) {
-        float ssum = 0.f, qsum = 0.f;
-#pragma unroll
-        for (int w = 0; w < 4 * neg; ++w) { ssum += slot[(w * 2 + 0) * 128 + px]; qsum += slot[(w * 2 + 1) * 128 + px]; }
-        atomicAdd(job.stats + px, (double)ssum);
-        atomicAdd(job.stats + job.Cout + px, (double)qsum);
-      }
-    }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (threadIdx.x == 0) {
-    trace_put(job, 3, trace_clock(job));
+  if (threadIdx.x == 0 && job.trace) {
+    trace_put(job, 3, clock64());
     int nu = 0;
     for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) ++nu;
     trace_put(job, 4, nu);
-  }
-  if (warp == 6) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)kTmemCols)
-                 : "memory");
   }
 }
 
 static size_t tc_fixed_smem(const ConvJob &job) {
   return (size_t)job.a_stages * 2 * job.stage16 * 16 + sizeof(TcShared) + 128 +
-         (job.xfold_kw ? (size_t)(job.mt >= 2 ? 2 : 1) * kTileM * kExchPitch * 4 :  // one exchange buffer per epilogue group that owns rows
-          (size_t)(256 + 8 * 2 * 128) * 4) + (job.nl ? (size_t)3 * kNlMaxC * 4 : 0);
+         (job.xfold_kw ? (size_t)kTileM * kExchPitch * 4 : (size_t)(256 + 8 * 2 * 128) * 4) + (job.nl ? (size_t)3 * kNlMaxC * 4 : 0);
 }
 size_t conv_tc_smem_bytes(const ConvJob &job) { return tc_fixed_smem(job) + (size_t)job.b_slots * job.chunk16 * 16; }
 
@@ -727,24 +424,43 @@ unsigned long long *conv_trace_claim(size_t words) {
 
 int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
   ConvJob job = job_in;
+  if (job.mt != 1 || job.rf_R || job.pf || job.ksplit) {
+    set_error("conv_tc: plan with mt=%d rf_R=%d pf=%d ksplit=%d has no wgmma kernel", job.mt, job.rf_R, job.pf, job.ksplit);
+    return FAV_ERR_UNSUPPORTED;
+  }
+  void (*kernel)(ConvJob) = nullptr;
+  switch (job.Npad) {
+    case 16: kernel = conv_tc_kernel<16>; break;
+    case 32: kernel = conv_tc_kernel<32>; break;
+    case 48: kernel = conv_tc_kernel<48>; break;
+    case 64: kernel = conv_tc_kernel<64>; break;
+    case 80: kernel = conv_tc_kernel<80>; break;
+    case 96: kernel = conv_tc_kernel<96>; break;
+    case 112: kernel = conv_tc_kernel<112>; break;
+    case 128: kernel = conv_tc_kernel<128>; break;
+    default:
+      set_error("conv_tc: no wgmma kernel for N = %d (multiples of 16 up to 128)", job.Npad);
+      return FAV_ERR_UNSUPPORTED;
+  }
   job.trace = conv_trace_claim((size_t)(job.ntiles < num_sms ? job.ntiles : num_sms) * kTraceWords);
   size_t smem = conv_tc_smem_bytes(job);
   if (smem > 227 * 1024) {
     set_error("conv_tc: shared memory %zu exceeds 227 KB", smem);
     return FAV_ERR_UNSUPPORTED;
   }
-  // the opt-in to > 48 KB of dynamic shared memory is a PER-DEVICE function attribute
-  static std::atomic<uint64_t> attr_set{0};
+  // the opt-in to > 48 KB of dynamic shared memory is a PER-DEVICE attribute of each instantiation
+  static std::atomic<uint64_t> attr_set[9];
   int dev = 0;
   FAV_TRY(check_cuda(cudaGetDevice(&dev), "cudaGetDevice"));
   const uint64_t bit = 1ull << (dev & 63);
-  if (!(attr_set.load(std::memory_order_acquire) & bit)) {
-    FAV_TRY(check_cuda(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
+  std::atomic<uint64_t> &set = attr_set[job.Npad / 16];
+  if (!(set.load(std::memory_order_acquire) & bit)) {
+    FAV_TRY(check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
                        "cudaFuncSetAttribute(conv_tc)"));
-    attr_set.fetch_or(bit, std::memory_order_release);
+    set.fetch_or(bit, std::memory_order_release);
   }
-  int grid = job.ntiles < num_sms ? job.ntiles : num_sms;
-  conv_tc_kernel<<<grid, kThreads, smem, st>>>(job);
+  const int grid = job.ntiles < num_sms ? job.ntiles : num_sms;
+  kernel<<<grid, job.nl ? kThreads : kConsumerThreads + 64, smem, st>>>(job);
   return post_launch("conv_tc");
 }
 

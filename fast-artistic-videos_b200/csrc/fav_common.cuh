@@ -1,4 +1,4 @@
-// fav_common.cuh -- shared helpers for libfav_b200 (sm_100a only).
+// fav_common.cuh -- shared helpers for libfav_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -49,7 +49,7 @@ __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; 
 __host__ __device__ inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 #ifdef __CUDACC__
-// The bilinear blend of BilinearSamplerBDHW.cu:103-106 exactly as nvcc (12.9, default -fmad=true, sm_100a) compiles the
+// The bilinear blend of BilinearSamplerBDHW.cu:103-106 exactly as nvcc (12.9, default -fmad=true, sm_90a) compiles the
 // reference kernel: the TR product is rounded, every other term is fused into the running sum (SASS: FMUL,FMUL,FMUL,FFMA,
 // FMUL,FMUL,FFMA,FFMA).  Pinned bit-for-bit against the reference's own kernel body compiled from /root/reference
 // (oracle/ref_warp/, tests/test_gpu_refwarp.py).  wx, wy = weights of the top-left corner, omx = 1 - wx, omy = 1 - wy.

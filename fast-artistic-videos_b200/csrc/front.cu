@@ -6,14 +6,14 @@
 //   a-8  fused 7-channel temporal input           fast_artistic_video_core.lua:161-171
 //   a-9  first-frame input                        fast_artistic_video_core.lua:133-137
 //
-// Design (B200): one thread owns VEC (=4) consecutive output pixels of one row so that the flow,
+// Design: one thread owns VEC (=4) consecutive output pixels of one row so that the flow,
 // cert and content reads and all stores are 16-byte vector accesses, fully coalesced (the reference
 // kernel maps lanes to x-stride-16 addresses and re-reads the flow once per channel).  The 4
 // bilinear taps are scalar read-only loads; for real optical flow neighbouring lanes gather
 // neighbouring addresses, so they coalesce in L1/L2 and each source sector is fetched from HBM once.
 // All arithmetic uses explicit round-to-nearest intrinsics in the reference's evaluation order.  The bilinear
 // blend reproduces the FMA contraction nvcc applies to the reference kernel (bilinear_ref_blend, fav_common.cuh), so the
-// warp is bit-identical to the reference's own CUDA kernel compiled for sm_100a (oracle/ref_warp) and to the CPU oracle.
+// warp is bit-identical to the reference's own CUDA kernel compiled for sm_90a (oracle/ref_warp) and to the CPU oracle.
 #include <algorithm>
 
 #include "fav_common.cuh"
@@ -332,7 +332,7 @@ __global__ void __launch_bounds__(256) temporal_input_kernel(
 
 // ---- the WHOLE temporal-consistency stage in one kernel ---------------------------------------------------------------
 // north star: "BilinearSamplerBDHW warp of the previous stylized frame by the supplied optical flow, consistencyChecker's
-// forward/backward-flow occlusion test, and the channel concat ... become one fused sm_100a kernel ... that writes the
+// forward/backward-flow occlusion test, and the channel concat ... become one fused sm_90a kernel ... that writes the
 // 7-channel tensor the net consumes directly".  Per 64 x 16 pixel tile (256 threads x 4 pixels):
 //   1. certainty of the tile + a (r/2)-pixel halo into shared memory: MODE 0 = the occlusion test itself
 //      (consistencyChecker.cpp:99-125, 3-argument mode; flow1 = the backward flow that also drives the warp, flow2 = forward

@@ -13,7 +13,6 @@
 #include <cstring>
 
 #include "conv_plan.hpp"
-#include "conv_res_plan.hpp"
 
 namespace fav {
 
@@ -67,7 +66,6 @@ struct PlanStep {
   int shave = 2;
   RawTensor raw;
   std::vector<ConvJob> tc;
-  std::vector<ResJob> res;   // non-empty: the tcgen05 path of this step is conv_res.cu (raw output planar)
   std::vector<SimtJob> simt;
   int stats_off = 0;
   int layer_index = -1;  // arch token index whose output this step completes (for fav_net_layer_output)
@@ -261,23 +259,6 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
     s.final_mode = last ? 1 : 0; s.out3 = out3; s.tanh_c = net->tanh_c;
     st.simt.push_back(s);
   }
-  if (st.raw.planar) {  // residual-block kernel (conv_res.cu): cost-balanced tile table, same packed weights as conv_tc
-    const ConvPhase &ph = c.phases[0];
-    ResJob r;
-    FAV_TRY(fill_res_job(c, ph, in, r));
-    ResPlan rp = plan_res_tiles(r.Ho, r.Wo, net->num_sms);
-    void *d_tiles = nullptr, *d_first = nullptr;
-    FAV_TRY(check_cuda(cudaMalloc(&d_tiles, rp.tiles.size() * sizeof(ResTile)), "cudaMalloc(res tiles)"));
-    pl.allocs.push_back(d_tiles);
-    FAV_TRY(check_cuda(cudaMalloc(&d_first, rp.cta_first.size() * sizeof(int)), "cudaMalloc(res tiles)"));
-    pl.allocs.push_back(d_first);
-    FAV_TRY(check_cuda(cudaMemcpy(d_tiles, rp.tiles.data(), rp.tiles.size() * sizeof(ResTile), cudaMemcpyHostToDevice), "cudaMemcpy(res tiles)"));
-    FAV_TRY(check_cuda(cudaMemcpy(d_first, rp.cta_first.data(), rp.cta_first.size() * sizeof(int), cudaMemcpyHostToDevice), "cudaMemcpy(res tiles)"));
-    r.tiles = (const ResTile *)d_tiles; r.cta_first = (const int *)d_first; r.grid = rp.grid;
-    r.b = ph.d_b_tc; r.bias = c.d_bias;
-    r.raw = st.raw.p; r.raw_Hp = st.raw.Hp; r.raw_Wp = st.raw.Wp;
-    st.res.push_back(r);
-  }
   return FAV_OK;
 }
 
@@ -357,10 +338,6 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       cs.raw.p = (pos & 1) ? pl->raw_buf2 : pl->raw_buf; cs.raw.C = c.cout; cs.raw.Cq = round_up(c.cout, 4) / 4; cs.raw.H = ho; cs.raw.W = wo;
       cs.raw.Hp = ho + 2; cs.raw.Wp = round_up(wo, kTileM);
       const bool last = op.last && i == n - 1;
-      if (!last && !getenv("FAV_NO_RES")) {  // residual-block convolutions: swapped-role kernel, planar raw output
-        ConvDef &cm = net->convs[op.conv[i]];
-        if (cm.phases.size() == 1 && conv_res_eligible(cm, cm.phases[0])) { cs.raw.planar = 1; cs.raw.Wp = round_up(wo, 16); }
-      }
       FAV_TRY(build_conv_jobs(net, *pl, cs, c, last, nullptr));
       // second conv of a residual block: fold the preceding InstanceNorm + ReLU pass into its patch producers
       if (op.kind == 1 && i == 1 && !pl->steps.empty() && pl->steps.back().kind == 1 && !getenv("FAV_NO_NL")) {
@@ -368,27 +345,12 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
         const InDef &n = net->inorms[ap.inorm];
         const Operand &in = pl->ops[cs.src];
         bool ok = ap.skip < 0 && n.C <= 256 && cs.tc.size() == 1;
-        if (ok && !cs.res.empty()) {  // conv_res.cu reads the PLANAR raw output of the block's first conv
-          ok = ap.raw.planar && n.C == pl->ops[cs.src].C;
-          if (ok) {
-            ResJob &r = cs.res[0];
-            const Operand &in = pl->ops[cs.src];
-            r.nl = 1; r.nl_pad = c.pad; r.nl_raw = ap.raw.p; r.nl_Hp = ap.raw.Hp; r.nl_Wp = ap.raw.Wp; r.nl_H = ap.raw.H; r.nl_W = ap.raw.W;
-            r.nl_relu = ap.relu; r.nl_C = n.C; r.nl_sums = pl->stats + ap.stats_off; r.nl_gamma = n.d_gamma; r.nl_beta = n.d_beta;
-            r.nl_inv_count = 1.0 / ((double)ap.raw.H * ap.raw.W); r.nl_eps = 1e-5;
-            (void)in;
-            ap.fused_nl = true;
-          }
-        } else if (ok && ap.raw.planar) {
-          ok = false;  // conv_tc's norm-on-load reads the quad layout only
-        } else
         if (ok) {
           ConvJob &j = cs.tc[0];
           ok = !j.rf_R && !j.pf && !j.xfold_kw && j.nseg == 1 && j.seg_dst16[0] == 0 && j.seg_len16[0] == j.pslab16 && j.row_mul == 1;
           if (ok) {
             ConvJob t = j;
             t.nl = 1;
-            if (const char *e = getenv("FAV_NL_MODE")) t.nl = atoi(e) == 2 ? 2 : 1;
             t.nl_raw = reinterpret_cast<const float4 *>(ap.raw.p); t.nl_Cq = ap.raw.Cq; t.nl_Wp = ap.raw.Wp;
             t.nl_H = ap.raw.H; t.nl_W = ap.raw.W; t.nl_padT = in.padT; t.nl_padL = in.padL; t.nl_relu = ap.relu; t.nl_C = n.C;
             t.nl_sums = pl->stats + ap.stats_off; t.nl_gamma = n.d_gamma; t.nl_beta = n.d_beta;
@@ -410,7 +372,6 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       PlanStep ns;
       ns.kind = 1; ns.inorm = op.inorm[i]; ns.raw = raw; ns.stats_off = stats_off;
       for (ConvJob &j : pl->steps.back().tc) j.stats = pl->stats + stats_off;  // statistics fused into the epilogue
-      for (ResJob &j : pl->steps.back().res) j.stats = pl->stats + stats_off;
       stats_off += 2 * c.cout;
       const ConvDef *consumer = pos + 1 < order.size() ? &net->convs[order[pos + 1]] : nullptr;
       FAV_TRY(make_operand(*pl, c.cout, ho, wo, consumer, &ns.dst));
@@ -472,9 +433,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
         double px = c.transposed ? (double)in.H * in.W : (double)s.raw.H * s.raw.W;
         FAV_TRY(begin(1, 2.0 * c.cin * c.cout * c.k * c.k * px, c.name));
       }
-      if (net->conv_impl == 0 && !s.res.empty()) {
-        for (ResJob &j : s.res) FAV_TRY(launch_conv_res(j, st));
-      } else if (net->conv_impl == 0) {
+      if (net->conv_impl == 0) {
         for (ConvJob &j : s.tc) {
           if (j.final_mode) { j.final_mode = final_mode; j.out3 = out3; }
           FAV_TRY(launch_conv_tc(j, net->num_sms, st));
@@ -648,7 +607,7 @@ int fav_net_create(const char *arch, const char *padding_type, float tanh_consta
       needs_bn = false; op.relu = c0 == 'C';  // :107-108, :113-114
       if (!zero_pad) shrink += 4 * scale;
     } else {
-      set_error("arch token '%s' is not supported by the sm_100a path (supported: cXsY-Z, fXsY-Z, dX, uX, UX, CX, RX)", v.c_str());
+      set_error("arch token '%s' is not supported by the sm_90a path (supported: cXsY-Z, fXsY-Z, dX, uX, UX, CX, RX)", v.c_str());
       return FAV_ERR_UNSUPPORTED;
     }
     if (op.last) { needs_bn = false; op.relu = false; }  // :117-120
@@ -701,8 +660,8 @@ int fav_net_finalize(fav_net_t *net) {
   cudaDeviceProp prop;
   FAV_TRY(check_cuda(cudaGetDevice(&net->device), "cudaGetDevice"));
   FAV_TRY(check_cuda(cudaGetDeviceProperties(&prop, net->device), "cudaGetDeviceProperties"));
-  if (prop.major != 10) {
-    set_error("libfav_b200 targets sm_100a (B200); device is sm_%d%d", prop.major, prop.minor);
+  if (prop.major != 9) {
+    set_error("libfav_b200 targets sm_90a (H100); device is sm_%d%d", prop.major, prop.minor);
     return FAV_ERR_UNSUPPORTED;
   }
   net->num_sms = prop.multiProcessorCount;

@@ -120,7 +120,7 @@ __global__ void __launch_bounds__(128) in_apply_kernel(RawTensor raw, const doub
   for (int it = 0; it < ITER; ++it) {
     const int x = xbase + it * 128;
     if (x < raw.W) {
-      if (raw.planar) {  // output of conv_res.cu: one plane per channel, lanes run along x (128-byte coalesced per plane)
+      if (raw.planar) {  // planar raw tensor: one plane per channel, lanes run along x (128-byte coalesced per plane)
         const float *p0 = raw.p + raw.offp(cb * 8, y, x);
         const int64_t plane = (int64_t)raw.Hp * raw.Wp;
 #pragma unroll

@@ -1,7 +1,7 @@
 // net_layout.cuh -- HBM data layouts of the stylization net (fast_artistic_video/models_video.lua:55-140).
 //
 // The reference keeps every activation as fp32 NCHW.  Internally this implementation uses two layouts,
-// both chosen so that the tcgen05 implicit-GEMM convolution needs neither im2col nor swizzled TMA maps:
+// both chosen so that the wgmma implicit-GEMM convolution needs neither im2col nor swizzled TMA maps:
 //
 //  Operand  activation feeding a convolution, stored as an fp16 PAIR (hi, lo) with x ~= hi + lo
 //           (22 significant bits).  Layout per tensor: [Hs][Cb][Ws][8 channels] -- 16 bytes per
@@ -13,9 +13,8 @@
 //           Inputs of stride-2 convolutions are stored parity-split: [Hs][Cb][2][Ws2][8]
 //           (even x plane, then odd x plane) so that stride-2 taps stay contiguous.
 //  Raw      fp32 convolution output before InstanceNorm: [Ho][Cq][Wp][4 channels] -- 16 bytes per
-//           (pixel, channel-quad); the epilogue thread that owns TMEM lane = pixel writes float4s that are
-//           coalesced across the 32 lanes of a warp.  The residual-block kernel (conv_res.cu: TMEM lane = output
-//           channel) writes PLANAR fp32 [C][Hp][Wp] instead (RawTensor::planar).
+//           (pixel, channel-quad); the epilogue writes the two channels a thread holds as one 8-byte store.
+//           RawTensor::planar (fp32 [C][Hp][Wp]) is a layout the normalisation kernels also accept.
 #pragma once
 #include "fav_common.cuh"
 #include <cuda_fp16.h>
@@ -77,7 +76,7 @@ struct RawTensor {
   int C = 0, Cq = 0;  // channels, channel quads
   int H = 0, W = 0;   // logical size
   int Hp = 0, Wp = 0; // allocated rows / row pitch in pixels (multiple of 128; planar: multiple of 16)
-  int planar = 0;     // 1: fp32 [C][Hp][Wp] (output of conv_res.cu, one channel per TMEM lane); 0: [Ho][Cq][Wp][4]
+  int planar = 0;     // 1: fp32 [C][Hp][Wp]; 0: [Ho][Cq][Wp][4]
   __host__ __device__ int64_t off4(int y, int cq, int x) const { return (((int64_t)y * Cq + cq) * Wp + x); }
   __host__ __device__ int64_t offp(int c, int y, int x) const { return (((int64_t)c * Hp + y) * Wp + x); }
 };

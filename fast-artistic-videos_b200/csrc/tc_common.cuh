@@ -1,5 +1,5 @@
-// tc_common.cuh -- inline-PTX helpers shared by the tcgen05 kernels (conv_tc.cu, conv_res.cu): mbarriers, bulk async copies,
-// tcgen05 fences / commit / MMA / TMEM loads.  sm_100a only.
+// tc_common.cuh -- inline-PTX helpers of the tensor-core convolution kernel (conv_tc.cu): mbarriers and bulk async
+// copies.  sm_90a.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,48 +43,4 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, fp16 inputs, fp32 accumulate
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// K-major, no swizzle: canonical layout ((8,m),(8 elems,2)) : ((16 B, SBO), (2 B, LBO))   [cute/atom/mma_traits_sm100.hpp]
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo16, uint32_t sbo16) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)(lbo16 & 0x3FFF) << 16) |
-         ((uint64_t)(sbo16 & 0x3FFF) << 32) | (1ull << 46) /* descriptor version: Blackwell */;
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// two 16-column loads in flight, one wait (single asm statement: no use of the registers can be scheduled before the wait)
-__device__ __forceinline__ void tmem_ld16x2(uint32_t ta, uint32_t tb, uint32_t (&r)[16], uint32_t (&q)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%32];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%33];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(q[0]), "=r"(q[1]),
-        "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]), "=r"(q[9]), "=r"(q[10]),
-        "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15])
-      : "r"(ta), "r"(tb)
-      : "memory");
-}
-
 }  // namespace fav

@@ -1,6 +1,6 @@
 // video_pipeline.cu -- f-2: the file-driven frame loop of fast_artistic_video.lua:93-170 as a native host pipeline around the
 // host-buffer session (session.cu).  The reference decodes, uploads, stylizes, downloads and encodes one frame after the other
-// (image.load / flowFile.load in interpreted Lua, image.save); at B200 speeds that host work bounds the frame rate by two
+// (image.load / flowFile.load in interpreted Lua, image.save); at H100 speeds that host work bounds the frame rate by two
 // orders of magnitude.  Here:
 //   decoder threads   read the PAYLOADS of frame PPM, certainty PGM and Middlebury .flo straight into PINNED ring slots
 //                     (cudaHostAlloc); byte -> fp32 / 255, 1 - cert, (u,v) -> (dy,dx) planes happen on the GPU behind the H2D

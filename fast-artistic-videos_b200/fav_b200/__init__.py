@@ -1,5 +1,5 @@
 """fav_b200 -- host-side mirror of the reference's operator surface for the per-frame video-style-transfer
-hot path, over the C ABI of libfav_b200.so (include/fav.h).  sm_100a only; no CPU fallback.
+hot path, over the C ABI of libfav_b200.so (include/fav.h).  sm_90a only; no CPU fallback.
 
   stn.BilinearSamplerBDHW          <- stnbdhw/BilinearSamplerBDHW.lua
   utils.warp_image / min_filter    <- fast_artistic_video/utils.lua

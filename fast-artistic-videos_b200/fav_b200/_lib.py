@@ -33,7 +33,7 @@ class FavError(RuntimeError):
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "or fast-artistic-videos_b200/build.sh (nvcc, sm_100a). There is no CPU fallback."
+        "or fast-artistic-videos_b200/build.sh (nvcc, sm_90a). There is no CPU fallback."
     )
 
 lib = C.CDLL(LIB_PATH)

@@ -1,6 +1,6 @@
 """fast_artistic_video/models_video.lua -- `models_video.build_model(opt)` (:55-140).
 
-Returns a StyleNet whose `forward(input[1x7xHxW]) -> [1x3xHxW]` runs the sm_100a path
+Returns a StyleNet whose `forward(input[1x7xHxW]) -> [1x3xHxW]` runs the sm_90a path
 (fav_net_forward, include/fav.h).  Parameters are addressed by the names listed in fav.h.
 """
 from __future__ import annotations

@@ -181,7 +181,7 @@ class Driver:
 # and write its PNG.  Filename patterns ([%d] / {%d}) and the wait-for-file protocol of the flow / occlusion producers
 # (utils.lua:74-80) are those of the synchronous driver; the PNGs are bit-identical to it (tests/test_gpu_net.py).
 # The reference decodes, uploads, computes, downloads and encodes strictly one after the other
-# (fast_artistic_video.lua:93-170); at B200 speeds that host work, not the GPU, bounds the frame rate.
+# (fast_artistic_video.lua:93-170); at H100 speeds that host work, not the GPU, bounds the frame rate.
 # ---------------------------------------------------------------------------------------------------------------------
 def _read_planes(path: str, channels: int, out: torch.Tensor) -> None:
     """image.load(path, channels) into a preallocated (pinned) [C,H,W] tensor."""

@@ -1,5 +1,5 @@
 /*
- * fav.h -- C ABI of libfav_b200.so: the B200-native (sm_100a) replacement for the per-frame
+ * fav.h -- C ABI of libfav_b200.so: the H100-native (sm_90a) replacement for the per-frame
  * video-style-transfer hot path of manuelruder/fast-artistic-videos (reference @ bf1d072).
  *
  * Plain C: raw DEVICE pointers (unless a parameter says "host"), sizes, element strides and a
@@ -36,7 +36,7 @@ enum {
   FAV_ERR_CUDA = 2,            /* cudaGetLastError() != success (BilinearSamplerBDHW.cu:146-150)   */
   FAV_ERR_NOT_IMPLEMENTED = 3, /* gradient entry points (BilinearSamplerBDHW.cu:171-184)           */
   FAV_ERR_IO = 4,
-  FAV_ERR_UNSUPPORTED = 5,     /* arch token / device the sm_100a path does not cover              */
+  FAV_ERR_UNSUPPORTED = 5,     /* arch token / device the sm_90a path does not cover              */
   FAV_ERR_NO_DEVICE = 6        /* no CUDA device: there is NO CPU fallback, calls fail loudly      */
 };
 
@@ -187,9 +187,9 @@ FAV_API int fav_net_num_params(const fav_net_t *net);
 FAV_API int fav_net_param_info(const fav_net_t *net, int index, char *name_out, int64_t shape_out[4],
                                int64_t *numel);
 FAV_API int fav_net_set_param(fav_net_t *net, const char *name, const float *host_data, int64_t numel);
-/* upload + repack weights for the tcgen05 path; must be called once after all set_param calls */
+/* upload + repack weights for the tensor-core path; must be called once after all set_param calls */
 FAV_API int fav_net_finalize(fav_net_t *net);
-/* conv implementation: 0 = tcgen05 implicit GEMM (default), 1 = CUDA-core debug comparator */
+/* conv implementation: 0 = tensor-core (wgmma) implicit GEMM (default), 1 = CUDA-core debug comparator */
 FAV_API int fav_net_set_conv_impl(fav_net_t *net, int impl);
 /* model:forward(input)                          fast_artistic_video_core.lua:138,172
  * in7 [in_dim,H,W] device fp32 -> out3 [3,H,W] device fp32 in net space (before deprocess). */
@@ -205,8 +205,8 @@ FAV_API int fav_net_profile(fav_net_t *net, const float *in7, int H, int W, floa
 FAV_API int fav_net_layer_output(fav_net_t *net, int index, float *out, int *C, int *Hl, int *Wl,
                                  void *stream);
 
-/* diagnostics (tools/trace_conv.py): per-CTA timeline of the following tcgen05 convolution launches (clock64 marks of
- * the MMA / epilogue warps, 64 u64 words per CTA, launches appended) into a caller-owned DEVICE buffer; NULL = off. */
+/* diagnostics: per-CTA timeline of the following tensor-core convolution launches (entry / set-up /
+ * exit clock64 marks, 64 u64 words per CTA, launches appended) into a caller-owned DEVICE buffer; NULL = off. */
 FAV_API int fav_debug_set_trace(void *dev_buf, size_t bytes);
 FAV_API size_t fav_debug_trace_words(void);
 

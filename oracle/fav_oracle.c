@@ -15,7 +15,7 @@
  *   - orc_warp_bdhw restates stnbdhw/BilinearSamplerBDHW.cu:13-32,58-108 line
  *     by line, including the FMA contraction nvcc applies to :103-106.  Pinned: the
  *     reference's kernel body, extracted from /root/reference at build time and
- *     compiled for sm_100a by oracle/Makefile (oracle/_ref/libref_warp.so), is
+ *     compiled for sm_90a by oracle/Makefile (oracle/_ref/libref_warp.so), is
  *     bit-identical to the CUDA product on the GPU box (tests/test_gpu_refwarp.py),
  *     and its outputs on seeded inputs are committed as tests/golden/warp_ref_*.npz,
  *     which this restatement reproduces bit for bit (tests/test_oracle.py).
@@ -86,7 +86,7 @@ ORC_API void orc_warp_bdhw(const float *img, const int64_t is[4], const float *g
           if (tr) vtr = p[(int64_t)y0 * is[2] + (int64_t)(x0 + 1) * is[3]];       /* :99 */
           if (bl) vbl = p[(int64_t)(y0 + 1) * is[2] + (int64_t)x0 * is[3]];       /* :100 */
           if (br) vbr = p[(int64_t)(y0 + 1) * is[2] + (int64_t)(x0 + 1) * is[3]]; /* :101 */
-          /* :103-106 as nvcc contracts it (12.9, default -fmad=true, sm_100a; SASS of the reference kernel body:
+          /* :103-106 as nvcc contracts it (12.9, default -fmad=true, sm_90a; SASS of the reference kernel body:
            * FMUL,FMUL,FMUL,FFMA,FMUL,FMUL,FFMA,FFMA): the TR product is rounded, the other three terms are fused
            * into the running sum.  Pinned against the compiled reference kernel (oracle/ref_warp, tests/golden/warp_ref_*). */
           float omx = 1 - wx, omy = 1 - wy;

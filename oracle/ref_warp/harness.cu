@@ -3,7 +3,7 @@
 // Wraps the reference's own CUDA kernel BilinearSamplerBDHW_bilinearSamplingFromGrid in a plain C entry point.
 // The kernel body is NOT in this repository: oracle/Makefile extracts lines 6-32 (stride_t + device helpers) and 48-109
 // (the __global__ kernel) of /root/reference/stnbdhw/BilinearSamplerBDHW.cu into oracle/_ref/ref_warp_kernel.inc at
-// build time and compiles this file for sm_100a with nvcc's default flags (the reference's CMakeLists.txt:55 adds only
+// build time and compiles this file for sm_90a with nvcc's default flags (the reference's CMakeLists.txt:55 adds only
 // an -arch flag, so FMA contraction is on, as here).  The launch configuration below is the reference launcher's
 // (BilinearSamplerBDHW.cu:119-120): blocks (C, Hout * ceil(Wout / 512), B), threads (32, 16).
 #include <cuda_runtime.h>

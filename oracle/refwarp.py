@@ -1,5 +1,5 @@
 """ctypes binding of oracle/_ref/libref_warp.so: the REFERENCE's own CUDA warp kernel
-(stnbdhw/BilinearSamplerBDHW.cu:48-109), extracted and compiled for sm_100a by oracle/Makefile behind
+(stnbdhw/BilinearSamplerBDHW.cu:48-109), extracted and compiled for sm_90a by oracle/Makefile behind
 oracle/ref_warp/harness.cu.  TEST INFRASTRUCTURE ONLY: the pin of the warp oracle (tests/) and the "kernel to beat"
 that bench.py times beside the product's warp.  Needs a CUDA device."""
 from __future__ import annotations

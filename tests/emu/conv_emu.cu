@@ -11,7 +11,6 @@
 #include <vector>
 
 #include "../../fast-artistic-videos_b200/csrc/conv_plan.hpp"
-#include "../../fast-artistic-videos_b200/csrc/conv_res_plan.hpp"
 
 namespace fav {
 static char g_err[512];
@@ -94,12 +93,12 @@ extern "C" int emu_conv_check(int cin, int cout, int k, int stride, int pad, int
     const int Npad = j.Npad;
     std::vector<uint16_t> st_hi((size_t)j.stage16 * 8), st_lo((size_t)j.stage16 * 8);
     std::vector<double> acc(j.rf_R ? (size_t)kTileM * 512 : (size_t)2 * kTileM * Npad);
-    std::vector<double> acc2(acc.size());  // K-split: the second issuing warp's accumulator (TMEM columns +128)
+    std::vector<double> acc2(acc.size());  // K-split: the second issuing warp's accumulator (columns +128)
     if (j.ksplit && (j.rf_R ? j.rf_R * j.rf_nblk : Npad) > 128) { set_error("ksplit needs <= 128 columns"); return 10; }
     if (j.ksplit && j.mt != 1 && !j.rf_R) { set_error("ksplit with mt = 2"); return 10; }
     for (int tile = 0; tile < j.ntiles; ++tile) {
       const int y = (tile / j.tiles_x) * j.mt, x0 = (tile % j.tiles_x) * j.tile_dx;
-      const double poison = (j.rf_R || j.ksplit) ? 1e30 : 0.0;  // stale TMEM must be overwritten, not accumulated
+      const double poison = (j.rf_R || j.ksplit) ? 1e30 : 0.0;  // a stale accumulator must be overwritten, not accumulated
       std::fill(acc.begin(), acc.end(), poison);
       std::fill(acc2.begin(), acc2.end(), poison);
       bool first_w[2] = {true, true};  // K-split: first MMA of each issuing warp in the unit (accumulate = 0)
@@ -366,146 +365,5 @@ extern "C" int emu_plan_detail(int cin, int cout, int k, int stride, int pad, in
   const int v[16] = {j.ngroups, j.nchunks, j.spc, j.nrows, j.CbG, j.nseg, j.a_stages, j.b_slots, j.b_resident, j.stage16 * 16,
                      j.chunk16 * 16, j.pslab16, j.tiles_x, j.ntiles, j.Npad, j.ksplit};
   for (int i = 0; i < 16; ++i) out16[i] = v[i];
-  return 0;
-}
-
-// ---- conv_res.cu (swapped roles: weights = M operand, pixels = N operand, cost-balanced tile table) ---------------------
-// Emulates the kernel's addressing from the same host planner (conv_res_plan.hpp): bulk-copy sources, stage layout, the two
-// matrix descriptors per K step, accumulator rows / columns, planar output placement; checks it against a direct convolution
-// and that every output pixel is produced exactly once.  info4 = {grid, tiles, max CTA cost, sum of CTA costs}.
-extern "C" int emu_res_check(int cin, int pad, int H, int W, int nctas, unsigned seed, double *max_err, double *max_ref, int *info4) {
-  const int cout = 128, k = 3;
-  ConvDef c;
-  init_conv_def(c, "emu_res", cin, cout, k, 1, pad, false, 0);
-  build_phases(c);
-  ConvPhase &ph = c.phases[0];
-  if (build_phase_tables(c, ph) != FAV_OK) return 1;
-  if (!conv_res_eligible(c, ph)) { set_error("layer not eligible for the residual kernel"); return 2; }
-  std::mt19937 rng(seed);
-  std::uniform_real_distribution<float> U(-1.f, 1.f);
-  std::vector<float> w((size_t)cin * cout * k * k), x((size_t)cin * H * W);
-  for (auto &v : w) v = U(rng) * 0.1f;
-  for (auto &v : x) v = U(rng) * 3.f;
-  Operand op = operand_geometry(cin, H, W, &c);
-  std::vector<uint16_t> hi(op.elems16 * 8, 0), lo(op.elems16 * 8, 0);
-  std::vector<float> xq((size_t)cin * H * W);
-  for (int ci = 0; ci < cin; ++ci)
-    for (int y = 0; y < H; ++y)
-      for (int xx = 0; xx < W; ++xx) {
-        float v = x[((size_t)ci * H + y) * W + xx];
-        uint16_t hb = f2h_bits(v), lb = f2h_bits(v - h2f_bits(hb));
-        int64_t o = op.off16(op.padT + y, ci / 8, op.padL + xx) * 8 + ci % 8;
-        hi[o] = hb; lo[o] = lb;
-        xq[((size_t)ci * H + y) * W + xx] = h2f_bits(hb) + h2f_bits(lb);
-      }
-  std::vector<uint16_t> pk = pack_phase_weights(c, ph, w);
-  ResJob j;
-  if (fill_res_job(c, ph, op, j) != FAV_OK) return 3;
-  const int Ho = j.Ho, Wo = j.Wo;
-  ResPlan pl = plan_res_tiles(Ho, Wo, nctas);
-  if ((int)pl.cta_first.size() != pl.grid + 1 || pl.cta_first.back() != (int)pl.tiles.size()) { set_error("tile table shape"); return 4; }
-  const int Wp = round_up(Wo, 16);
-  std::vector<double> out((size_t)cout * Ho * Wp, 0.0);
-  std::vector<int> written((size_t)Ho * Wo, 0);
-  const size_t stage16 = (size_t)4 * kResCbG * kResPslab;  // one plane
-  const size_t chunk16 = (size_t)2 * kResSpc * 2 * 128;
-  std::vector<uint16_t> st_hi(stage16 * 8), st_lo(stage16 * 8);
-  std::vector<double> acc((size_t)2 * 128 * kResMaxNt);
-  for (int cta = 0; cta < pl.grid; ++cta) {
-    if (pl.cta_first[cta + 1] <= pl.cta_first[cta]) { set_error("CTA %d has no tile", cta); return 5; }
-    for (int ti = pl.cta_first[cta]; ti < pl.cta_first[cta + 1]; ++ti) {
-      const ResTile t = pl.tiles[ti];
-      if (t.nt <= 0 || t.nt > kResMaxNt || t.nt % 16 || t.x0 % 16 || t.y % 2 || t.y >= Ho || t.x0 >= Wo) { set_error("bad tile"); return 6; }
-      std::fill(acc.begin(), acc.end(), 1e30);  // stale TMEM must be overwritten by the first MMA (accumulate = 0)
-      bool first = true;
-      for (int g = 0; g < j.ngroups; ++g) {
-        std::fill(st_hi.begin(), st_hi.end(), (uint16_t)0x7e00);  // NaN poison: reading an unloaded byte is a bug
-        std::fill(st_lo.begin(), st_lo.end(), (uint16_t)0x7e00);
-        for (int lane = 0; lane < 4 * kResCbG * 2; ++lane) {  // the producer warp: lane = (patch row, channel block, hi/lo)
-          const int ri = lane / (2 * kResCbG), cbi = (lane >> 1) % kResCbG, part = lane & 1;
-          const int64_t src16 = ((int64_t)(t.y + ri + j.in_row0) * j.a_Cb + g * kResCbG + cbi) * j.a_slab16 + t.x0 + j.in_col0;
-          const int64_t dst16 = (int64_t)(ri * kResCbG + cbi) * kResPslab, len16 = t.nt + 2;
-          if (src16 < 0 || src16 + len16 > (int64_t)op.elems16) { set_error("src OOB"); return 7; }
-          if (dst16 + len16 > (int64_t)stage16) { set_error("dst OOB"); return 8; }
-          std::vector<uint16_t> &dstv = part ? st_lo : st_hi;
-          const std::vector<uint16_t> &srcv = part ? lo : hi;
-          for (int64_t e = 0; e < len16 * 8; ++e) dstv[dst16 * 8 + e] = srcv[src16 * 8 + e];
-        }
-        int sidx = 0;
-        for (int ch = 0; ch < kResChunks; ++ch) {
-          const uint16_t *chunk = pk.data() + ((size_t)g * kResChunks + ch) * chunk16 * 8;
-          for (int st = 0; st < kResSpc; ++st, ++sidx) {
-            const uint32_t dls = j.steps[sidx];
-            const int a_off16 = dls & 0xffff, lbo16 = dls >> 16;
-            for (int r = 0; r < 2; ++r)
-              for (int u = 0; u < 2; ++u)
-                for (int m = 0; m < 128; ++m) {
-                  const int64_t w16 = (int64_t)st * 256 + (int64_t)u * 128 + m;  // LBO = 128 rows, SBO: 8-row groups contiguous
-                  const uint16_t *wh = chunk + w16 * 8, *wl = chunk + ((int64_t)kResSpc * 256 + w16) * 8;
-                  for (int n = 0; n < t.nt; ++n) {
-                    const int64_t p16 = (int64_t)r * kResCbG * kResPslab + a_off16 + (int64_t)u * lbo16 + n;
-                    if (p16 >= (int64_t)stage16) { set_error("patch descriptor OOB"); return 9; }
-                    double d = (first && u == 0) ? 0.0 : acc[((size_t)r * 128 + m) * kResMaxNt + n];
-                    for (int i = 0; i < 8; ++i) {
-                      const double a_h = h2f_bits(wh[i]), a_l = h2f_bits(wl[i]);
-                      const double b_h = h2f_bits(st_hi[p16 * 8 + i]), b_l = h2f_bits(st_lo[p16 * 8 + i]);
-                      d += a_h * b_h + a_l * b_h + a_h * b_l;
-                    }
-                    acc[((size_t)r * 128 + m) * kResMaxNt + n] = d;
-                  }
-                }
-            first = false;
-          }
-        }
-      }
-      for (int r = 0; r < 2; ++r) {
-        const int yo = t.y + r;
-        if (yo >= Ho) continue;
-        for (int n = 0; n < t.nt; ++n) {
-          if (t.x0 + n >= Wp) { set_error("store beyond the row pitch"); return 10; }
-          if (t.x0 + n < Wo) written[(size_t)yo * Wo + t.x0 + n]++;
-          for (int m = 0; m < cout; ++m) out[((size_t)m * Ho + yo) * Wp + t.x0 + n] = acc[((size_t)r * 128 + m) * kResMaxNt + n];
-        }
-      }
-    }
-  }
-  for (int wv : written)
-    if (wv != 1) { set_error("output pixel written %d times", wv); return 11; }
-  double me = 0, mr = 0;
-  for (int co = 0; co < cout; ++co)
-    for (int oy = 0; oy < Ho; ++oy)
-      for (int ox = 0; ox < Wo; ++ox) {
-        double sref = 0;
-        for (int ci = 0; ci < cin; ++ci)
-          for (int ky = 0; ky < k; ++ky) {
-            int iy = oy + ky - pad;
-            if (iy < 0 || iy >= H) continue;
-            for (int kx = 0; kx < k; ++kx) {
-              int ix = ox + kx - pad;
-              if (ix < 0 || ix >= W) continue;
-              sref += (double)w[(((size_t)co * cin + ci) * k + ky) * k + kx] * xq[((size_t)ci * H + iy) * W + ix];
-            }
-          }
-        double dv = std::fabs(out[((size_t)co * Ho + oy) * Wp + ox] - sref);
-        if (!(dv <= 1e300)) dv = 1e300;
-        me = std::max(me, dv); mr = std::max(mr, std::fabs(sref));
-      }
-  *max_err = me; *max_ref = mr;
-  if (info4) { info4[0] = pl.grid; info4[1] = (int)pl.tiles.size(); info4[2] = pl.max_cost; info4[3] = pl.sum_cost; }
-  return 0;
-}
-
-// tile-table statistics only (full-size layers): info6 = {grid, tiles, max cost, sum cost, narrowest tile, widest tile}
-extern "C" int emu_res_plan(int Ho, int Wo, int nctas, int *info6) {
-  ResPlan pl = plan_res_tiles(Ho, Wo, nctas);
-  std::vector<int> cover((size_t)((Ho + 1) / 2) * ((Wo + 15) / 16), 0);
-  int mn = 1 << 30, mx = 0;
-  for (const ResTile &t : pl.tiles) {
-    mn = std::min(mn, (int)t.nt); mx = std::max(mx, (int)t.nt);
-    for (int g = 0; g < t.nt / 16; ++g) cover[(size_t)(t.y / 2) * ((Wo + 15) / 16) + t.x0 / 16 + g]++;
-  }
-  for (int v : cover)
-    if (v != 1) { set_error("granule covered %d times", v); return 1; }
-  info6[0] = pl.grid; info6[1] = (int)pl.tiles.size(); info6[2] = pl.max_cost; info6[3] = pl.sum_cost; info6[4] = mn; info6[5] = mx;
   return 0;
 }

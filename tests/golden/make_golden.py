@@ -1,8 +1,8 @@
-"""Generates the committed golden fixtures under tests/golden/ (run HERE, where /root/reference exists).
+"""Generates the committed golden fixtures under tests/golden/ (run where the reference sources are present).
 
   consistency_*.npz : seeded flow pairs (+ frame) and the {0,255} masks written by the REFERENCE's own
                       consistencyChecker binary (oracle/_ref/consistencyChecker, compiled unmodified from
-                      /root/reference/consistencyChecker by oracle/Makefile), 3- and 4-argument mode.
+                      the reference consistencyChecker by oracle/Makefile), 3- and 4-argument mode.
   clip_64x96.npz    : fp64 PyTorch-oracle outputs of a 3-frame synthetic clip (net + recurrence);
                       the torch restatement is "parity unpinned" (Torch7 cannot run here), see DESIGN.md.
 Inputs are regenerated from seeds by fav_b200.synth at test time; only outputs are stored.

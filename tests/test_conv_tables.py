@@ -1,4 +1,4 @@
-"""CPU emulation of the tcgen05 kernel's addressing (tests/emu/conv_emu.cu) against a direct convolution, for every
+"""CPU emulation of the wgmma kernel's addressing (tests/emu/conv_emu.cu) against a direct convolution, for every
 layer shape of the supported archs plus edge shapes: validates K-step tables, patch segments, parity-split input,
 sub-pixel phases of the transposed convolution, weight packing and the fp16 hi/lo split (3-MMA scheme)."""
 import ctypes as C
@@ -17,7 +17,7 @@ def emu():
     so = os.path.join(EMU, "libfav_emu.so")
     src = os.path.join(EMU, "conv_emu.cu")
     csrc = os.path.join(ROOT, "fast-artistic-videos_b200", "csrc")
-    hdrs = [os.path.join(csrc, h) for h in ("conv_plan.hpp", "conv_res_plan.hpp", "conv_res.cuh", "conv.cuh")]
+    hdrs = [os.path.join(csrc, h) for h in ("conv_plan.hpp", "conv.cuh")]
     if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(f) for f in [src] + hdrs):
         subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
                                "-Wno-deprecated-gpu-targets", "-o", so, src])
@@ -66,57 +66,20 @@ def plan(emu, *case):
 
 
 def test_planner_decisions_for_the_720p_layers(emu):
-    """The plans DESIGN.md section 4.1 describes, at the sizes of the 720p frame."""
+    """The plans conv_tc.cu runs (DESIGN.md section 4.1), at the sizes of the 720p frame: one output row per unit, one
+    register accumulator of N <= 128 columns per warpgroup (no two-row units, K-split, row-fold or phase-fold)."""
     res = plan(emu, 128, 128, 3, 1, 0, 0, 0, 180, 320)
-    assert res["mt"] == 2 and not res["ksplit"] and not res["b_resident"]            # two-row units, one issuing warp per row
+    assert res["mt"] == 1 and not res["ksplit"] and not res["b_resident"] and res["Npad"] == 128   # weights stream through the ring
     conv1 = plan(emu, 7, 32, 9, 1, 4, 0, 0, 800, 1360)
-    assert conv1["rf_R"] == 4 and conv1["ksplit"] and conv1["b_resident"]            # row-fold + K-split
+    assert conv1["rf_R"] == 0 and conv1["b_resident"] and conv1["Npad"] == 32
     final = plan(emu, 32, 3, 9, 1, 4, 0, 0, 720, 1280)
-    assert final["rf_R"] == 8 and final["xfold_kw"] == 9 and not final["ksplit"]     # x-fold + 8-row fold (256 columns)
+    assert final["rf_R"] == 0 and final["xfold_kw"] == 9 and final["Npad"] == 32        # x-fold: N = 9 x 3 -> 32
     u64 = plan(emu, 128, 64, 3, 2, 1, 1, 1, 180, 320)
-    assert u64["pf"] and u64["Npad"] == 256 and not u64["ksplit"]                    # phase-fold, N = 4 x 64
+    assert not u64["pf"] and u64["Npad"] == 64                                          # four sub-pixel phase jobs
     u32 = plan(emu, 64, 32, 3, 2, 1, 1, 1, 360, 640)
-    assert u32["pf"] and u32["Npad"] == 128 and u32["ksplit"] and u32["b_resident"]
-    final64 = plan(emu, 64, 3, 9, 1, 4, 0, 0, 720, 1280)                             # paper arch: 64 input channels
-    assert final64["rf_R"] == 0 and final64["xfold_kw"] == 9                         # 35 KB patch rows: x-fold only (row-fold measured 2.3x slower)
+    assert not u32["pf"] and u32["Npad"] == 32 and u32["b_resident"]
+    final64 = plan(emu, 64, 3, 9, 1, 4, 0, 0, 720, 1280)                                # paper arch: 64 input channels
+    assert final64["rf_R"] == 0 and final64["xfold_kw"] == 9
     for case in ((32, 64, 3, 2, 1, 0, 0, 800, 1360), (64, 128, 3, 2, 1, 0, 0, 400, 680)):
         d = plan(emu, *case)
-        assert d["mt"] == 1 and d["ksplit"]
-
-
-# ---- conv_res.cu: swapped-role residual kernel, cost-balanced tile table ---------------------------------------------------
-RES_CASES = [  # cin, pad, H, W, nctas
-    (128, 0, 6, 134, 148),    # fewer granules than CTAs
-    (128, 0, 7, 320, 148),    # odd output row count (second row of the last pair missing), 318-px rows
-    (128, 0, 14, 340, 12),    # several tiles per CTA, cuts inside rows, 338-px rows (last granule 2 px wide)
-    (128, 0, 11, 100, 5),
-    (128, 1, 5, 130, 7),      # zero-padded variant (c3s1-128)
-    (64, 0, 6, 70, 3),        # two channel groups
-    (128, 0, 3, 3, 148),      # 1x1 output
-]
-
-
-@pytest.mark.parametrize("case", RES_CASES)
-def test_emulated_residual_kernel_matches_direct_conv(emu, case):
-    me, mr = C.c_double(), C.c_double()
-    info = (C.c_int * 4)()
-    rc = emu.emu_res_check(*case, 3, C.byref(me), C.byref(mr), info)
-    assert rc == 0, emu.emu_last_error().decode()
-    assert me.value <= 2e-6 * max(mr.value, 1.0), (me.value, mr.value)
-
-
-@pytest.mark.parametrize("shape", [(198, 338), (196, 336), (180, 320), (288, 498), (270, 480), (560 - 2, 980 - 2), (532 - 2, 532 - 2)])
-def test_residual_tile_table_is_balanced(emu, shape):
-    """Every granule exactly once; the most expensive CTA within 6 % of the mean (the first design gave 2 or 3 fixed 128-px
-    units per SM: up to 50 % imbalance at 297 units on 148 SMs).  198x338 is the one awkward 720p layer: 99 row pairs x 22
-    granules need 148.5 CTAs for a sliver-free 3-CTAs-per-2-row-pairs pattern, so ONE kind of CTA gets three tiles (6,6,1
-    granules, cost 163 vs 134); the rest must stay tight."""
-    info = (C.c_int * 6)()
-    assert emu.emu_res_plan(shape[0], shape[1], 148, info) == 0, emu.emu_last_error().decode()
-    grid, tiles, mx, sm, narrow, wide = list(info)
-    assert grid == 148 and wide <= 128
-    if shape == (198, 338):
-        assert mx <= 163 and sm / grid <= 136, (mx, sm / grid)
-    else:
-        assert mx <= 1.16 * sm / grid, (mx, sm / grid)  # row pairs of 20-22 granules vs 12-15 per CTA: a few whole-granule patterns only
-        assert narrow >= 48, narrow
+        assert d["mt"] == 1 and not d["ksplit"]

@@ -1,7 +1,8 @@
-"""Pins the warp against the REFERENCE ITSELF: the reference's own CUDA kernel (stnbdhw/BilinearSamplerBDHW.cu:48-109,
-compiled for sm_100a from /root/reference by oracle/Makefile into oracle/_ref/libref_warp.so, original (32,16) block /
-(C, H*ceil(W/512), B) grid) vs the product's fav_bilinear_sampler_bdhw_update_output / fused temporal input and vs the
-C oracle.  Bar: BIT-EXACT at every BASELINE.json config shape, real and stress flows, and on the committed vectors."""
+"""Pins the warp against the REFERENCE ITSELF: outputs of the reference's own CUDA kernel (stnbdhw/BilinearSamplerBDHW.cu:48-109,
+compiled for sm_90a behind oracle/ref_warp/harness.cu, original (32,16) block / (C, H*ceil(W/512), B) grid), recorded on an
+H100 by tests/golden/make_warp_golden.py into tests/golden/refwarp_cases.npz and warp_ref.npz, vs the product's
+fav_bilinear_sampler_bdhw_update_output / fused temporal input and vs the C oracle.  Bar: BIT-EXACT (SHA-256 of every
+output) at every BASELINE.json config shape, real and stress flows, and on the committed vectors."""
 import os
 import sys
 
@@ -10,12 +11,11 @@ import pytest
 import torch
 
 from conftest import ROOT
-from fav_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-import make_warp_golden  # noqa: E402
+import make_warp_golden as mwg  # noqa: E402
 
 
 def T(a):
@@ -23,80 +23,55 @@ def T(a):
 
 
 @pytest.fixture(scope="module")
-def ref():
-    from oracle import refwarp
-
-    assert refwarp.available(), "oracle/_ref/libref_warp.so must travel to the GPU box (built by `make -C oracle refwarp`)"
-    return refwarp
+def gold():
+    return np.load(os.path.join(ROOT, "tests", "golden", "refwarp_cases.npz"))
 
 
-def _ulp_diff(a, b):
-    ia, ib = a.view(np.int32).astype(np.int64), b.view(np.int32).astype(np.int64)
-    ia = np.where(ia < 0, -(ia & 0x7FFFFFFF), ia); ib = np.where(ib < 0, -(ib & 0x7FFFFFFF), ib)
-    return int(np.abs(ia - ib).max())
-
-
-# the five BASELINE.json config shapes (256^2 tiny, 720p, 1080p, 2048^2 VR face, 4K) + ragged small ones
-SHAPES = [(256, 256), (720, 1280), (1080, 1920), (2048, 2048), (2160, 3840), (97, 75), (33, 129)]
-
-
-@pytest.mark.parametrize("shape", SHAPES)
-def test_product_warp_equals_reference_kernel(ref, shape):
-    import fav_b200
+@pytest.mark.parametrize("shape", mwg.REF_SHAPES)
+def test_product_warp_equals_reference_kernel(gold, shape):
     from fav_b200 import utils
 
     H, W = shape
-    img = T(synth.make_frame(H, W, 1) * 1.2 - 0.1)
-    for name, flow in (("real", synth.checker_to_lua(synth.make_backward_flow(H, W, 2))), ("stress", synth.stress_flow(H, W))):
-        f = T(flow)
-        r = ref.warp(img[None], f[None])[0]
-        g = utils.warp_image(img, f)
-        torch.cuda.synchronize()
-        if not torch.equal(r, g):
-            pytest.fail(f"{shape} {name}: {int((r != g).sum())} differing values, max ulp "
-                        f"{_ulp_diff(r.cpu().numpy(), g.cpu().numpy())}")
+    img, flows = mwg.shape_inputs(H, W)
+    for name, flow in flows.items():
+        g = utils.warp_image(T(img), T(flow)).cpu().numpy()
+        key = f"{H}x{W}_{name}"
+        if mwg.digest(g) != str(gold[key + "_sha"]):
+            want, got = gold[key + "_sample"], g.reshape(-1)[mwg.sample_index(g.size)]
+            pytest.fail(f"{shape} {name}: output differs from the reference kernel's; {int((want != got).sum())} of "
+                        f"{want.size} sampled values differ")
 
 
-def test_reference_kernel_batch_channels_and_output_size(ref):
+def test_reference_kernel_batch_channels_and_output_size(gold):
     from fav_b200 import stn
 
-    rng = np.random.default_rng(0)
-    img = T(rng.uniform(size=(2, 5, 20, 28)).astype(np.float32))
-    grid = T(rng.uniform(-6, 6, size=(2, 2, 13, 36)).astype(np.float32))
-    assert torch.equal(ref.warp(img, grid), stn.BilinearSamplerBDHW().forward((img, grid)))
+    img, grid = mwg.batch_inputs()
+    assert np.array_equal(stn.BilinearSamplerBDHW().forward((T(img), T(grid))).cpu().numpy(), gold["batch"])
     g = torch.full((1, 2, 20, 28), 99999.0, device="cuda")  # sentinel flow of vr_helper.lua:10
-    assert float(ref.warp(img[:1], g).abs().max()) == 0.0
+    assert float(np.abs(gold["sentinel"]).max()) == 0.0
+    assert np.array_equal(stn.BilinearSamplerBDHW().forward((T(img[:1]), g)).cpu().numpy(), gold["sentinel"])
 
 
-def test_fused_temporal_input_prior_equals_reference_kernel_composition(ref):
+def test_fused_temporal_input_prior_equals_reference_kernel_composition(gold):
     """in[3:6] of the fused kernel == preprocess(reference-kernel warp) * cert composed with torch ops in the
     reference's op order (core.lua:166-167), bit for bit."""
     from fav_b200 import _lib
-    from oracle import net_oracle
 
-    H, W = 360, 640
-    c, p = T(synth.make_frame(H, W, 2)), T(synth.make_frame(H, W, 1) * 1.2 - 0.1)
-    flow = T(synth.checker_to_lua(synth.make_backward_flow(H, W, 2)))
-    cert = T(net_oracle.make_cert(H, W, 2))
+    c, p, flow, cert = (T(a) for a in mwg.prior_inputs())
+    H, W = c.shape[-2:]
     out = torch.empty((7, H, W), device="cuda")
     _lib.check(_lib.lib.fav_temporal_input(_lib.dptr(c), _lib.dptr(p), _lib.dptr(flow), _lib.dptr(cert), None, None,
                                            _lib.dptr(out), H, W, 0, _lib.stream_ptr()))
-    warped = ref.warp(p[None], flow[None])[0]
-    mean = torch.tensor([103.939, 116.779, 123.68], device="cuda").view(3, 1, 1)
-    pre = warped[[2, 1, 0]] * 255.0 - mean           # preprocess.lua:57-62: index, mul(255), add(-1, mean)
-    prior = torch.zeros_like(pre) + pre * cert       # core.lua:167 fill(vgg-mean = 0) + cmul
-    assert torch.equal(out[3:6], prior)
+    assert mwg.digest(out[3:6].cpu().numpy()) == str(gold["prior_360x640_sha"])
 
 
-def test_oracle_and_product_reproduce_committed_reference_vectors(ref):
-    """tests/golden/warp_ref.npz was written by this very kernel on a B200 (make_warp_golden.py); re-derive it live."""
+def test_oracle_and_product_reproduce_committed_reference_vectors():
+    """tests/golden/warp_ref.npz was written by the reference kernel (make_warp_golden.py)."""
     from fav_b200 import stn
     from oracle import pyoracle
 
     gold = np.load(os.path.join(ROOT, "tests", "golden", "warp_ref.npz"))
-    for case in make_warp_golden.WARP_CASES:
-        img, flow = make_warp_golden.warp_inputs(case)
-        live = ref.warp(T(img)[None], T(flow)[None])[0].cpu().numpy()
-        assert np.array_equal(live, gold[case[0]]), case[0]
-        assert np.array_equal(stn.BilinearSamplerBDHW().forward((T(img), T(flow))).cpu().numpy(), live), case[0]
-        assert np.array_equal(pyoracle.warp_bdhw(img, flow), live), case[0]
+    for case in mwg.WARP_CASES:
+        img, flow = mwg.warp_inputs(case)
+        assert np.array_equal(stn.BilinearSamplerBDHW().forward((T(img), T(flow))).cpu().numpy(), gold[case[0]]), case[0]
+        assert np.array_equal(pyoracle.warp_bdhw(img, flow), gold[case[0]]), case[0]

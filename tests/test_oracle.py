@@ -54,7 +54,7 @@ def test_consistency_oracle_equals_reference_binary_live(tmp_path):
 
 def test_warp_oracle_reproduces_reference_kernel_vectors():
     """tests/golden/warp_ref.npz = outputs of the REFERENCE's own CUDA kernel (stnbdhw/BilinearSamplerBDHW.cu:48-109 compiled
-    for sm_100a, oracle/ref_warp) on a B200, written by tests/golden/make_warp_golden.py: the C restatement (including the
+    for sm_90a, oracle/ref_warp) on an H100, written by tests/golden/make_warp_golden.py: the C restatement (including the
     FMA contraction of :103-106) must reproduce them bit for bit -- this pins orc_warp_bdhw with the reference itself."""
     import make_warp_golden
 

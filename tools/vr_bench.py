@@ -1,5 +1,5 @@
 """BASELINE.json configs[3]: 360-degree VR cube-map path (fast_artistic_video_vr.lua), 2048 px per face (overlap included),
-mosaic model (paper arch), 1 x B200: VR frames/s END TO END through the driver mirror (fav_b200.vr): per VR frame 6 faces with
+mosaic model (paper arch), 1 x H100: VR frames/s END TO END through the driver mirror (fav_b200.vr): per VR frame 6 faces with
 border priors (perspective warps of already stylized neighbours), flow-warped previous face, fused re-blend of all six faces,
 3x3 median, cube map + equirectangular output (PNG encode excluded by -no_png timing split: reported both ways)."""
 import json, os, shutil, sys, time
