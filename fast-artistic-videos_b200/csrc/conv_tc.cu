@@ -82,6 +82,9 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x, ++tl) {
     if (job.b_resident) sb = 0;
     uint32_t scale = 0;
+    // one chunk of wgmmas stays in flight while the next is issued: a weight slot is released once the following chunk
+    // is committed and the slot's own chunk has completed, a patch stage once the last chunk that read it has completed
+    uint32_t b_prev = 0, a_prev = 0;
     for (int g = 0; g < ngroups; ++g) {
       mbar_wait(&sh->a_full[sa], aph);
       // A descriptor start: pixel r of the patch is at +16 B * r, this warpgroup's rows begin 64 pixels in
@@ -102,13 +105,22 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
           scale = 1;
         }
         wgmma_commit();
-        wgmma_wait<0>();  // the slot's operands are consumed: release it
-        if (!job.b_resident && wt == 0) mbar_arrive(&sh->b_empty[sb]);
+        wgmma_wait<1>();  // every chunk but this one has completed
+        if ((g | c) && wt == 0) {
+          if (!job.b_resident) mbar_arrive(&sh->b_empty[b_prev]);
+          if (c == 0) mbar_arrive(&sh->a_empty[a_prev]);
+        }
+        b_prev = sb;
         sidx += (uint32_t)spc;
         if (++sb == nslots) { sb = 0; bph ^= 1; }
       }
-      if (wt == 0) mbar_arrive(&sh->a_empty[sa]);
+      a_prev = sa;
       if (++sa == nstages) { sa = 0; aph ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (wt == 0) {
+      if (!job.b_resident) mbar_arrive(&sh->b_empty[b_prev]);
+      mbar_arrive(&sh->a_empty[a_prev]);
     }
     if (job.dbg & 8) continue;
 

@@ -17,25 +17,30 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// Bounded wait: a protocol bug must surface as a trap (launch failure), never as a hung GPU.
+// Bounded wait: a protocol bug must surface as a trap (launch failure), never as a hung GPU.  The loop is written in
+// PTX as one block: the same loop in C++ leaves the consumers a divergent path while wgmmas are in flight, and ptxas
+// then serialises them (C7518).
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  uint32_t done = 0;
-  const uint32_t addr = smem_u32(bar);
-  long long t0 = 0;
-  for (uint32_t spin = 0; !done; ++spin) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (!done && (spin & 255u) == 255u) {
-      long long now = clock64();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000ll) __trap();  // ~2 s at 2 GHz
-    }
-  }
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b32 spin;\n\t.reg .b64 t0, now;\n\t"
+      "mov.u32 spin, 0;\n\tmov.u64 t0, 0;\n"
+      "LAB_WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@p bra LAB_DONE;\n\t"
+      "add.u32 spin, spin, 1;\n\t"
+      "and.b32 spin, spin, 255;\n\t"
+      "setp.ne.u32 p, spin, 0;\n\t"
+      "@p bra LAB_WAIT;\n\t"
+      "mov.u64 now, %%clock64;\n\t"
+      "setp.eq.u64 p, t0, 0;\n\t"
+      "@p mov.u64 t0, now;\n\t"
+      "sub.s64 now, now, t0;\n\t"
+      "setp.gt.s64 p, now, 4000000000;\n\t"  // ~2 s at 2 GHz
+      "@p trap;\n\t"
+      "bra LAB_WAIT;\n"
+      "LAB_DONE:\n\t}" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
 }
 __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
