@@ -8,7 +8,8 @@ constexpr int kMaxTaps = 81;
 constexpr int kMaxSteps = 168;
 constexpr int kMaxRfRows = 24;  // row-fold: R + KH - 1 patch rows per unit
 constexpr int kMaxRows = 10;
-constexpr int kMaxGroups = 12;
+constexpr int kMaxGroups = 16;  // K groups of one job: Cin = 512 in channel groups of 4 blocks (VGG-16 conv4_x)
+constexpr int kMaxNBlock = 128;  // output channels of one job (wgmma N); wider convolutions run one job per N block
 constexpr int kTileM = 128;  // output pixels per tile (two 64-row wgmma halves)
 constexpr int kTraceWords = 64;   // u64 words per CTA in the optional timeline buffer
 constexpr int kTraceUnits = 6;    // units (tiles) per CTA recorded

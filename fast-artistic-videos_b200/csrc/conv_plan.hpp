@@ -340,6 +340,20 @@ static inline void init_conv_def(ConvDef &c, const std::string &name, int cin, i
   c.out_mul = tr ? stride : 1;
 }
 
+// ---- N blocks: a plain convolution with Cout > kMaxNBlock runs as ceil(Cout / 128) jobs of <= 128 output channels each.
+// Block b is an ordinary convolution over every input channel with output channels [128 b, 128 b + cout_b): its own
+// ConvDef (so its own tables and packed weights), a bias slice, and a raw output pointer advanced by 128 b channels
+// (32 b channel quads of the [Ho][Cq][Wp][4] layout; the row pitch Cq stays the full tensor's).
+static inline int conv_nblocks(int cout) { return (cout + kMaxNBlock - 1) / kMaxNBlock; }
+static inline int conv_nblock_cout(int cout, int b) { return std::min(kMaxNBlock, cout - b * kMaxNBlock); }
+// weights [Cout][Cin][k][k] -> the [cout_b][Cin][k][k] slice of block b
+static inline std::vector<float> conv_nblock_weights(const std::vector<float> &w, int cin, int cout, int k, int b) {
+  const size_t per = (size_t)cin * k * k;
+  const size_t c0 = (size_t)b * kMaxNBlock, n = (size_t)conv_nblock_cout(cout, b);
+  return std::vector<float>(w.begin() + c0 * per, w.begin() + (c0 + n) * per);
+}
+static inline int64_t conv_nblock_raw_offset(int b, int raw_Wp) { return (int64_t)b * (kMaxNBlock / 4) * raw_Wp * 4; }
+
 // packed tcgen05 weights of one phase: [group][chunk][hi|lo][step][k8 half][Npad][8] fp16 (as uint16 bit patterns)
 static inline std::vector<uint16_t> pack_phase_weights(const ConvDef &c, const ConvPhase &ph, const std::vector<float> &w) {
   if (ph.rf_R) {

@@ -84,6 +84,16 @@ SIGNATURES = {
     "fav_net_profile": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_float),
                                   C.POINTER(C.c_double), C.c_char_p, C.POINTER(C.c_int), _fp]),
     "fav_net_layer_output": (C.c_int, [C.c_void_p, C.c_int, _fp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), _fp]),
+    "fav_percep_create": (C.c_int, [C.c_int, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_double), C.c_int,
+                                    C.POINTER(C.c_int), C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_void_p)]),
+    "fav_percep_destroy": (None, [C.c_void_p]),
+    "fav_percep_set_conv": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]),
+    "fav_percep_finalize": (C.c_int, [C.c_void_p]),
+    "fav_percep_set_style_target": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp]),
+    "fav_percep_evaluate": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), _fp]),
+    "fav_percep_layer_output": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                          C.POINTER(C.c_int), _fp]),
+    "fav_percep_style_stat": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), _fp]),
     "fav_debug_set_trace": (C.c_int, [_fp, C.c_size_t]),
     "fav_debug_trace_words": (C.c_size_t, []),
     "fav_run_image": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, _fp, _fp]),

@@ -10,8 +10,9 @@ Differences that are design, not semantics:
     (weights 1,0,0,0);
   * `generate_fill` (:108-117) draws torch.rand even when the result is discarded ('vgg-mean'); here nothing is drawn
     for 'vgg-mean' and 'uniform-random' draws on the GPU (the reference RNG stream is not reproducible anyway).
--evaluate (:76-98,214-239): the temporal loss is computed (utils.temporal_loss, one fused kernel); the perceptual
-style / content terms need the VGG-16 loss network (models/vgg16.t7, no network here) and are reported as NaN.
+-evaluate (:76-98,214-239): the temporal loss is computed (utils.temporal_loss, one fused kernel); the content and style losses
+run through the loss network on the GPU (fav_b200/percep.py) when -loss_network names one or models/vgg16.t7 exists, and are
+reported as NaN otherwise.
 """
 from __future__ import annotations
 
@@ -63,6 +64,40 @@ def load_model(path_or_style: str, arch: str = synth.DEFAULT_ARCH, in_dim: int =
     return models_video.synthetic_model(style, arch, in_dim)
 
 
+def make_evaluate_image(opt):
+    """The perceptual-loss set-up of core.lua:74-98 and evaluate_image (:101-106), or None when no loss network is available
+    (-loss_network not given and no models/vgg16.t7).  A -loss_network or -style_image that was named and is missing is an
+    I/O error."""
+    import os
+
+    from . import percep
+
+    path = _opt(opt, "loss_network", None)
+    if path in (None, ""):
+        path = os.path.join("models", "vgg16.t7")
+        if not os.path.exists(path):
+            return None
+    elif not os.path.exists(path):
+        raise _lib.FavError(_lib.FAV_ERR_IO, f"-loss_network {path}: no such file")
+    content_layers, content_weights = percep.parse_layers(_opt(opt, "content_layers", "16"), _opt(opt, "content_weights", "1.0"))
+    style_layers, style_weights = percep.parse_layers(_opt(opt, "style_layers", "4,9,16,23"), _opt(opt, "style_weights", "1.0"))
+    crit = percep.PerceptualCriterion.from_t7(path, content_layers, content_weights, style_layers, style_weights,
+                                              _opt(opt, "style_target_type", "gram"))
+    style_path = _opt(opt, "style_image", "images/styles/candy.jpg")
+    if not os.path.exists(style_path):
+        raise _lib.FavError(_lib.FAV_ERR_IO, f"-style_image {style_path}: no such file")
+    from .video import load_image  # image.load(opt.style_image, 3, 'float')
+
+    style = percep.scale_style_image(load_image(style_path, 3), int(_opt(opt, "style_image_size", 256)))
+    crit.set_style_target(style.cuda())
+
+    def evaluate_image(content_img, stylized_img):
+        return crit.evaluate(content_img, stylized_img)
+
+    evaluate_image.criterion = crit
+    return evaluate_image
+
+
 def run_fast_neural_video(opt, func_load_image, func_load_cert, func_eval, func_make_last_frame_warped,
                           func_is_single_image, func_save_image, model_vid=None, model_img=None):
     dtype = "torch.CudaTensor"  # utils.setup_gpu (utils.lua:43-66): this implementation is GPU-only
@@ -76,6 +111,7 @@ def run_fast_neural_video(opt, func_load_image, func_load_cert, func_eval, func_
     model_img = model_img if model_img is not None else (
         None if _opt(opt, "model_img", "self") in ("self", "", None)
         else load_model(_opt(opt, "model_img"), _opt(opt, "arch_img", _opt(opt, "arch", synth.DEFAULT_ARCH)), in_dim=3))
+    evaluate_image = make_evaluate_image(opt) if evaluate else None
     fill_mode = _opt(opt, "fill_occlusions", "vgg-mean")
     assert fill_mode in ("vgg-mean", "uniform-random")
 
@@ -134,10 +170,9 @@ def run_fast_neural_video(opt, func_load_image, func_load_cert, func_eval, func_
             nxt = run_next_image(H, W, img, cert.reshape(1, 1, H, W), i)
         func_save_image(opt, i, nxt, dtype)
         if evaluate:
-            # core.lua:214-226: func_eval -> { style_loss, content_loss, temporal_loss }.  The perceptual terms need the VGG-16
-            # loss network (models/vgg16.t7, not available offline): func_eval is called with evaluate_image = None and reports
-            # NaN for them; the temporal term is computed (fused warp + mask + MSE kernel).
-            numbers, n_num = func_eval(opt, i, None, dtype)
+            # core.lua:214-226: func_eval -> { style_loss, content_loss, temporal_loss }; evaluate_image is None without a
+            # loss network (the perceptual terms are then NaN); the temporal term is one fused warp + mask + MSE kernel.
+            numbers, n_num = func_eval(opt, i, evaluate_image, dtype)
             for j in range(n_num):
                 if j >= len(eval_tabl):
                     eval_tabl.append([]); eval_sum.append(0.0)

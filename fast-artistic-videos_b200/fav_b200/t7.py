@@ -337,3 +337,89 @@ def write_checkpoint(path: str, arch: str, state: Dict[str, np.ndarray], tanh_co
     w.obj({"opt": {"arch": arch, "padding_type": padding_type}, "iter": 60000, "model": seq(mods)})
     with open(path, "wb") as f:
         f.write(bytes(w.b))
+
+
+# ---- loss network (-evaluate, -loss_network) ---------------------------------------------------------------------------
+# An nn.Sequential of SpatialConvolution[MM] / ReLU / SpatialMaxPooling (the nn.* or cudnn.* classes), as loadcaffe writes
+# VGG-16 (models/vgg16.t7, fast_artistic_video.lua:63).  PerceptualCriterion trims every module after the deepest loss layer
+# (layer_utils.lua:146-165), whatever its type, so VGG's classifier (View / Linear / Dropout / SoftMax) is never read.
+LOSS_MODULES = ("SpatialConvolution", "SpatialConvolutionMM", "ReLU", "SpatialMaxPooling")
+
+
+def _unsupported(msg):
+    from . import _lib
+
+    return _lib.FavError(_lib.FAV_ERR_UNSUPPORTED, msg)
+
+
+def loss_network_from_model(model, last_index: int) -> List[dict]:
+    """The first `last_index` top-level modules of a loss network as dicts: {'type': 'conv', cin, cout, k, stride, pad,
+    weight [cout,cin,k,k], bias}, {'type': 'relu'}, {'type': 'pool', kW, kH, dW, dH, padW, padH, ceil_mode}.  Any other module
+    before that index, and a convolution the tensor-core planner cannot run, raise FavError(FAV_ERR_UNSUPPORTED) naming the
+    module and its (1-based) index."""
+    mods = _mods(model)
+    if last_index > len(mods):
+        from . import _lib
+
+        raise _lib.FavError(_lib.FAV_ERR_INVALID, f"loss network: layer {last_index} requested, the network has {len(mods)} modules")
+    out = []
+    for i, m in enumerate(mods[:last_index], 1):
+        c = _cls(m)
+        name = m.torch_type if isinstance(m, T7Object) else type(m).__name__
+        if c not in LOSS_MODULES:
+            raise _unsupported(f"loss network module {i} ({name}): only SpatialConvolution, ReLU and SpatialMaxPooling are supported "
+                               "before the deepest loss layer")
+        if c.startswith("SpatialConvolution"):
+            cin, cout = int(m["nInputPlane"]), int(m["nOutputPlane"])
+            kw, kh, dw, dh = int(m["kW"]), int(m["kH"]), int(m["dW"]), int(m["dH"])
+            pw, ph = int(m.get("padW", 0)), int(m.get("padH", m.get("padW", 0)))
+            ok = (kw == kh and dw == dh and pw == ph and kw % 2 == 1 and pw <= kw // 2 and (cin <= 8 or cin % 16 == 0)
+                  and (dw == 1 or (dw == 2 and kw == 3 and pw == 1)) and m.get("groups", 1) in (1, None))
+            if not ok:
+                raise _unsupported(f"loss network module {i} ({name} {cin}->{cout}, kernel {kw}x{kh}, stride {dw}x{dh}, pad {pw}x{ph}): "
+                                   "not a convolution geometry the tensor-core planner runs")
+            w = np.asarray(m["weight"], np.float32).reshape(cout, cin, kw, kw)  # SpatialConvolutionMM stores [cout, cin*k*k]
+            out.append(dict(type="conv", cin=cin, cout=cout, k=kw, stride=dw, pad=pw, weight=np.ascontiguousarray(w),
+                            bias=np.asarray(m["bias"], np.float32).reshape(cout)))
+        elif c == "ReLU":
+            out.append(dict(type="relu"))
+        else:
+            out.append(dict(type="pool", kW=int(m["kW"]), kH=int(m["kH"]), dW=int(m["dW"]), dH=int(m["dH"]),
+                            padW=int(m.get("padW", 0)), padH=int(m.get("padH", 0)), ceil_mode=bool(m.get("ceil_mode", False))))
+    return out
+
+
+def load_loss_network(path: str, last_index: int) -> List[dict]:
+    """torch.load(opt.loss_network) (fast_artistic_video_core.lua:82), trimmed after module `last_index`."""
+    return loss_network_from_model(load(path), last_index)
+
+
+def write_loss_network(path: str, modules: List[dict], classifier: bool = True, cudnn: bool = False, conv_mm: bool = False) -> None:
+    """Serialise a loss network (the dicts of loss_network_from_model) as an nn.Sequential .t7 file.  classifier=True appends
+    VGG-16's head as loadcaffe names it (View, Linear, ReLU, Dropout, ..., SoftMax); trimming never reads it, so its Linear
+    modules carry 1x1 stand-in tensors instead of the 0.5 GB of real fc weights.  cudnn=True writes the cudnn.* classes,
+    conv_mm=True SpatialConvolutionMM with 2-D [cout, cin*k*k] weights."""
+    pre = "cudnn." if cudnn else "nn."
+    seq = []
+    for m in modules:
+        if m["type"] == "conv":
+            k = m["k"]
+            w = np.asarray(m["weight"], np.float32)
+            cls = "nn.SpatialConvolutionMM" if conv_mm else pre + "SpatialConvolution"
+            seq.append(T7Object(cls, {"nInputPlane": m["cin"], "nOutputPlane": m["cout"], "kW": k, "kH": k, "dW": m["stride"],
+                                      "dH": m["stride"], "padW": m["pad"], "padH": m["pad"],
+                                      "weight": w.reshape(m["cout"], -1) if conv_mm else w, "bias": np.asarray(m["bias"], np.float32)}))
+        elif m["type"] == "relu":
+            seq.append(T7Object(pre + "ReLU", {"inplace": True}))
+        else:
+            seq.append(T7Object(pre + "SpatialMaxPooling", {"kW": m["kW"], "kH": m["kH"], "dW": m["dW"], "dH": m["dH"],
+                                                            "padW": m["padW"], "padH": m["padH"], "ceil_mode": bool(m["ceil_mode"])}))
+    if classifier:
+        stand_in = lambda: {"weight": np.zeros((1, 1), np.float32), "bias": np.zeros((1,), np.float32)}
+        seq += [T7Object("nn.View", {"size": 25088}), T7Object("nn.Linear", stand_in()), T7Object("nn.ReLU", {"inplace": True}),
+                T7Object("nn.Dropout", {"p": 0.5}), T7Object("nn.Linear", stand_in()), T7Object("nn.ReLU", {"inplace": True}),
+                T7Object("nn.Dropout", {"p": 0.5}), T7Object("nn.Linear", stand_in()), T7Object("nn.SoftMax", {})]
+    w = _Writer()
+    w.obj(T7Object("nn.Sequential", {"modules": {i + 1: m for i, m in enumerate(seq)}}))
+    with open(path, "wb") as f:
+        f.write(bytes(w.b))

@@ -34,6 +34,10 @@ def build_parser():
     a("-evaluation_file", default="evaluation.txt"); a("-flow_pattern_eval", default=""); a("-occlusions_pattern_eval", default="")
     a("-invert_occlusion_eval", action="store_true"); a("-fix_occlusions_eval", action="store_true"); a("-backward_eval", action="store_true")
     a("-model_img_arch", default="")
+    # the perceptual terms of -evaluate (fast_artistic_video.lua:57-67); no -loss_network and no models/vgg16.t7: reported as nan
+    a("-content_weights", default="1.0"); a("-content_layers", default="16")
+    a("-loss_network", default=None); a("-style_image", default="images/styles/candy.jpg"); a("-style_image_size", type=int, default=256)
+    a("-style_weights", default="1.0"); a("-style_layers", default="4,9,16,23"); a("-style_target_type", default="gram", choices=["gram", "mean"])
     a("-pipeline", type=int, default=1)  # 1: threaded decode / encode around the host-buffer session (f-2); 0: synchronous driver
     a("-arch", default=core.synth.DEFAULT_ARCH)
     return p
@@ -149,15 +153,19 @@ class Driver:
         return flow, cert
 
     def func_eval(self, opt, i, func_percept_loss, dtype):  # :128-151
-        nan = float("nan")  # style / content loss: the VGG-16 loss network is not available (core.py)
+        # :129 unpacks evaluate_image's (content, style) pair as `style_loss, content_loss`, so the first row of the evaluation
+        # file holds the content losses and the second the style losses; reproduced as written.  Without a loss network
+        # (core.make_evaluate_image returns None) both are nan.
+        nan = float("nan")
+        style_loss, content_loss = func_percept_loss(self.last_frame, self.last_frame_stylized) if func_percept_loss else (nan, nan)
         if i > 1:
             flow_eval, cert_eval = self.func_load_flow_cert_eval(opt, i, dtype)
             if opt.backward_eval:
                 t = utils.temporal_loss(self.last_frame_stylized, self.prev_last_frame_stylized, flow_eval, cert_eval)
             else:
                 t = utils.temporal_loss(self.prev_last_frame_stylized, self.last_frame_stylized, flow_eval, cert_eval)
-            return [nan, nan, t], 3
-        return [nan, nan, 0.0], 3
+            return [style_loss, content_loss, t], 3
+        return [style_loss, content_loss, 0.0], 3
 
     def func_save_image(self, opt, i, img, dtype=None):  # :160-170
         out_path = "%s-%05d.png" % (opt.output_prefix, i)

@@ -205,6 +205,46 @@ FAV_API int fav_net_profile(fav_net_t *net, const float *in7, int H, int W, floa
 FAV_API int fav_net_layer_output(fav_net_t *net, int index, float *out, int *C, int *Hl, int *Wl,
                                  void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * f-5  the perceptual loss network of -evaluate: nn.PerceptualCriterion with nn.ContentLoss / nn.StyleLoss
+ *      (fast_artistic_video/PerceptualCriterion.lua:27-155, ContentLoss.lua:39-48, StyleLoss.lua:39-55,
+ *      GramMatrix.lua:31-53), set up as fast_artistic_video_core.lua:74-98 does.
+ * The loss network is a chain of modules, 8 ints each (module i of the file's nn.Sequential is entry i-1):
+ *   {0, nInputPlane, nOutputPlane, k, stride, pad, 0, 0}  SpatialConvolution (square kernel)
+ *   {1, 0, ...}                                            ReLU
+ *   {2, kW, kH, dW, dH, padW, padH, ceil_mode}             SpatialMaxPooling
+ * Layer indices are 1-based top-level module indices; the module's OUTPUT is the feature map (conv + bias, ReLU output,
+ * pooled map).  Modules after the deepest loss layer are dropped (layer_utils.lua:146-165).  agg_type: 0 'gram', 1 'mean'
+ * (-style_target_type, StyleLoss.lua:14-24).  FAV_ERR_UNSUPPORTED names the module of a geometry the tensor-core path does
+ * not run.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct fav_percep fav_percep_t;
+FAV_API int fav_percep_create(int n_modules, const int *modules8, int n_content, const int *content_layers,
+                              const double *content_weights, int n_style, const int *style_layers,
+                              const double *style_weights, int agg_type, fav_percep_t **out);
+FAV_API void fav_percep_destroy(fav_percep_t *p);
+/* weights of convolution module `module_index` (1-based): host fp32 [nOutputPlane, nInputPlane, k, k] and [nOutputPlane] */
+FAV_API int fav_percep_set_conv(fav_percep_t *p, int module_index, const float *weight, int64_t weight_numel,
+                                const float *bias, int64_t bias_numel);
+FAV_API int fav_percep_finalize(fav_percep_t *p);
+/* percep_crit:setStyleTarget(preprocess(style_image))      fast_artistic_video_core.lua:93-97, PerceptualCriterion.lua:72-80
+ * rgb [3,H,W] device fp32 in [0,1] (already scaled to -style_image_size by the caller); the VGG preprocess runs on the GPU. */
+FAV_API int fav_percep_set_style_target(fav_percep_t *p, const float *rgb, int H, int W, void *stream);
+/* evaluate_image(content, stylized)                        fast_artistic_video_core.lua:101-106
+ * content, stylized [3,H,W] device fp32 RGB [0,1] (stylized: the unclamped frame); returns total_content_loss and
+ * total_style_loss through HOST doubles (synchronises `stream`).  FAV_ERR_UNSUPPORTED if an activation left the fp16 operand
+ * range (|x| > 65504): the losses are then not computed from clamped values. */
+FAV_API int fav_percep_evaluate(fav_percep_t *p, const float *content, const float *stylized, int H, int W,
+                                double *content_loss, double *style_loss, void *stream);
+/* tests: feature map of loss layer `index` from the last forward, fp32 NCHW [C,Hl,Wl] (out may be NULL for the sizes).
+ * pass 0: the content-target forward of the last evaluation (content layers only); pass 1: the evaluated image, or the style
+ * image after fav_percep_set_style_target (PerceptualCriterion.lua:85-93,117-125). */
+FAV_API int fav_percep_layer_output(fav_percep_t *p, int pass, int index, float *out, int *C, int *Hl, int *Wl,
+                                    void *stream);
+/* tests: the aggregate (StyleLoss.lua:40-43) of style layer k (0-based position in the style layer list) as DEVICE
+ * doubles: Gram matrix C*C (GramMatrix.lua:31-53) or C means; which 0 = style target, 1 = last evaluated image. */
+FAV_API int fav_percep_style_stat(fav_percep_t *p, int which, int k, double *out, int *n, void *stream);
+
 /* diagnostics: per-CTA timeline of the following tensor-core convolution launches (entry / set-up /
  * exit clock64 marks, 64 u64 words per CTA, launches appended) into a caller-owned DEVICE buffer; NULL = off. */
 FAV_API int fav_debug_set_trace(void *dev_buf, size_t bytes);
