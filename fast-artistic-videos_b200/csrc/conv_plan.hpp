@@ -49,6 +49,10 @@ struct ConvDef {
   int in_stride = 1;  // stride of the input sampling grid (2 for 'd' layers)
   int tpad = 0;       // transposed: zero border the input operand needs (= -min tap offset over the sub-pixel phases)
   int out_mul = 1;    // 2 for transposed stride-2 (sub-pixel phases)
+  // the output is read back as raw [Ho][Cq][Wp][4] by the next kernel: every conv of the loss network and every conv of the
+  // stylization net but its last.  Such a conv never takes the x-fold plan, whose epilogue writes the net's final tanh image
+  // through ConvJob::out3 instead of the raw output.
+  bool raw_out = false;
   std::vector<ConvPhase> phases;
   ConvPhase fold;    // transposed conv: all 4 phases in one tcgen05 job (phase-fold); phases[] stay for the comparator
   bool has_fold = false;
@@ -81,7 +85,7 @@ static inline int build_phase_tables(const ConvDef &c, ConvPhase &ph) {
   };
   const int nrows = (int)ph.rows.size();
   ph.Npad = c.Npad;
-  const bool xfold = !c.transposed && c.in_stride == 1 && c.k >= 5 && c.cout <= 4 && c.Cb % 2 == 0 && c.pad == (c.k - 1) / 2;
+  const bool xfold = !c.raw_out && !c.transposed && c.in_stride == 1 && c.k >= 5 && c.cout <= 4 && c.Cb % 2 == 0 && c.pad == (c.k - 1) / 2;
   if (xfold) {
     ph.kind = 3; ph.Npad = round_up(c.k * c.cout, 16);
     ph.CbG = (c.Cb % 4 == 0) ? 4 : 2; ph.nchg = c.Cb / ph.CbG;
@@ -351,6 +355,12 @@ static inline std::vector<float> conv_nblock_weights(const std::vector<float> &w
   const size_t per = (size_t)cin * k * k;
   const size_t c0 = (size_t)b * kMaxNBlock, n = (size_t)conv_nblock_cout(cout, b);
   return std::vector<float>(w.begin() + c0 * per, w.begin() + (c0 + n) * per);
+}
+// the ConvDef of N block b of a loss-network convolution (raw output, so never the x-fold plan)
+static inline void init_nblock_conv_def(ConvDef &c, const std::string &name, int cin, int cout, int k, int stride, int pad, int b) {
+  init_conv_def(c, name, cin, conv_nblock_cout(cout, b), k, stride, pad, false, 0);
+  c.raw_out = true;
+  build_phases(c);
 }
 static inline int64_t conv_nblock_raw_offset(int b, int raw_Wp) { return (int64_t)b * (kMaxNBlock / 4) * raw_Wp * 4; }
 

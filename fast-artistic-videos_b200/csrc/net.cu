@@ -618,6 +618,11 @@ int fav_net_create(const char *arch, const char *padding_type, float tanh_consta
   FAV_REQUIRE(prev == 3, "the last layer must produce 3 channels (got %d)", prev);
   FAV_REQUIRE(net->ops.back().kind == 0 && !net->convs[net->ops.back().conv[0]].transposed,
               "the last arch token must be a (non-transposed) convolution");
+  if (scale != 1.0) {  // the final layer writes a [3][H][W] frame: a net that resizes the frame would write past it
+    set_error("arch '%s' resizes the frame by %g (its strided and upsampling layers must cancel)", arch, 1.0 / scale);
+    return FAV_ERR_UNSUPPORTED;
+  }
+  for (ConvDef &c : net->convs) c.raw_out = &c != &net->convs[net->ops.back().conv[0]];  // only the last may x-fold
   FAV_REQUIRE(shrink == std::floor(shrink) && ((int)shrink) % 2 == 0, "unsupported shrink %f", shrink);
   net->reflect_pad = (int)shrink / 2;  // train_video.lua:319-324
   *out = net.release();

@@ -14,8 +14,7 @@ extern "C" int emu_nblock_check(int cin, int cout, int k, int pad, int H, int W,
   for (auto &v : x) v = U(rng) * 3.f;
   const int nb = conv_nblocks(cout);
   ConvDef c0;
-  init_conv_def(c0, "emu", cin, conv_nblock_cout(cout, 0), k, 1, pad, false, 0);
-  build_phases(c0);
+  init_nblock_conv_def(c0, "emu", cin, cout, k, 1, pad, 0);
   Operand op = operand_geometry(cin, H, W, &c0);
   std::vector<uint16_t> hi(op.elems16 * 8, 0), lo(op.elems16 * 8, 0);
   std::vector<float> xq((size_t)cin * H * W);
@@ -36,8 +35,7 @@ extern "C" int emu_nblock_check(int cin, int cout, int k, int pad, int H, int W,
   int groups = 0;
   for (int b = 0; b < nb; ++b) {
     ConvDef c;
-    init_conv_def(c, "emu", cin, conv_nblock_cout(cout, b), k, 1, pad, false, 0);
-    build_phases(c);
+    init_nblock_conv_def(c, "emu", cin, cout, k, 1, pad, b);
     ConvPhase &ph = c.phases[0];
     if (build_phase_tables(c, ph) != FAV_OK) return 1;
     if (ph.kind != 0 && ph.kind != 1) { set_error("N-block job planned as kind %d", ph.kind); return 12; }

@@ -63,6 +63,12 @@ def test_arch_parser_and_param_table():
     with pytest.raises(Exception) as e:
         models_video.StyleNet("c9s1-32,X5,c9s1-3")
     assert "not supported" in str(e.value)
+    from fav_b200 import _lib
+
+    # one stride-2 layer, two upsampling ones: the net would return a 2H x 2W image, past the [3][H][W] output frame
+    with pytest.raises(_lib.FavError) as e:
+        models_video.StyleNet("c9s1-32,d64,R64,u32,u8,c9s1-3")
+    assert e.value.status == _lib.FAV_ERR_UNSUPPORTED and "resizes the frame by 2" in str(e.value)
 
 
 def test_no_cpu_fallback_without_device():

@@ -47,6 +47,11 @@ CASES = [  # cin, cout, k, stride, pad, transposed, adj, H, W
     (64, 32, 3, 1, 1, 1, 0, 6, 140),     # f3s1-32: stride-1 full convolution = convolution with the flipped filter
     (32, 16, 5, 2, 2, 1, 1, 5, 70),      # f5s2-16: four sub-pixel phases with 9/6/6/4 taps, tap offsets -1..1
     (64, 64, 3, 1, 1, 0, 0, 7, 150),     # residual conv of the 'zero' padding type (pad 1, 64 channels: conv_tc path)
+    (16, 3, 9, 1, 4, 0, 0, 6, 130),      # final c9s1-3 from 16 channels: x-fold with CbG 2
+    (32, 3, 5, 1, 2, 0, 0, 6, 260),      # final c5s1-3: x-fold with N = 5 x 3 -> 16, 124-px tile stride
+    (8, 3, 9, 1, 4, 0, 0, 6, 140),       # final conv from 8 channels: tap pairing, plain final epilogue
+    (32, 3, 3, 1, 1, 0, 0, 5, 129),      # final c3s1-3: generic plan, plain final epilogue
+    (32, 8, 3, 2, 1, 1, 1, 4, 70),       # u8: Cout 8 in an N = 16 instance
 ]
 
 
@@ -80,6 +85,9 @@ def test_planner_decisions_for_the_720p_layers(emu):
     assert not u32["pf"] and u32["Npad"] == 32 and u32["b_resident"]
     final64 = plan(emu, 64, 3, 9, 1, 4, 0, 0, 720, 1280)                                # paper arch: 64 input channels
     assert final64["rf_R"] == 0 and final64["xfold_kw"] == 9
+    assert plan(emu, 32, 3, 5, 1, 2, 0, 0, 720, 1280)["xfold_kw"] == 5                  # c5s1-3: N = 15 -> 16
+    for case in ((8, 3, 9, 1, 4, 0, 0, 720, 1280), (32, 3, 3, 1, 1, 0, 0, 720, 1280)):  # 8-channel input / 3x3: no x-fold
+        assert plan(emu, *case)["xfold_kw"] == 0
     for case in ((32, 64, 3, 2, 1, 0, 0, 800, 1360), (64, 128, 3, 2, 1, 0, 0, 400, 680)):
         d = plan(emu, *case)
         assert d["mt"] == 1 and not d["ksplit"]

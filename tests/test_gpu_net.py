@@ -37,7 +37,9 @@ def rand_input(H, W, seed=0):
     return x7.astype(np.float32)
 
 
-@pytest.mark.parametrize("shape", [(64, 96), (128, 200), (256, 256)])
+# 48x508 / 48x516: the residual convs output widths 127 ... 145 / 129 ... 147, so tiles end 1 pixel short of or 1 pixel into
+# a 128-pixel tile (H stays above the reflection pad of 40)
+@pytest.mark.parametrize("shape", [(64, 96), (128, 200), (256, 256), (48, 508), (48, 516)])
 @pytest.mark.parametrize("impl", ["tcgen05", "simt"])
 def test_net_forward_and_every_layer_vs_fp64_oracle(net, shape, impl):
     from oracle import net_oracle
@@ -87,6 +89,12 @@ def test_paper_arch_with_nearest_upsampling(shape):
     ("c9s1-32,d64,C64,R64,f3s2-32,f3s1-32,c9s1-3", "reflect-start"),   # CX block, fXsY-Z full convolutions (stride 2 and 1), 64-ch blocks
     ("c9s1-32,d64,d128,R128,R128,f5s2-64,u32,c9s1-3", "reflect-start"),  # 5x5 full convolution: 4 sub-pixel phases with 9/6/6/4 taps
     (synth.DEFAULT_ARCH, "zero"),                                       # padding_type zero: padded residual convs, Identity skip
+    # wgmma N = 16 / 48 / 80, a residual block with 10 channel blocks (CbG 2, norm-on-load), x-fold from 16 channels (CbG 2)
+    ("c9s1-16,d48,d80,R80,R80,u48,u16,c9s1-3", "reflect-start"),
+    ("c9s1-32,d96,d112,R112,u96,u32,c5s1-3", "reflect-start"),         # N = 96 / 112; x-fold c5s1-3 with N = 5 x 3 -> 16
+    ("c9s1-32,d64,d128,R128,u32,u8,c9s1-3", "reflect-start"),          # Cout 8 (N 16, padded IN statistics); final conv
+                                                                       # from 8 channels: tap pairing, plain final epilogue
+    ("c9s1-32,d64,R64,u32,c3s1-3", "zero"),                             # generic final conv (N = 16), plain final epilogue
 ])
 def test_arch_tokens_and_padding_types(arch, ptype):
     """models_video.build_model's remaining tokens (fXsY-Z :81-89, CX :103-108) and padding_type 'zero' (:13-19,46-50) vs the

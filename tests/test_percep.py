@@ -1,5 +1,6 @@
 """-evaluate's perceptual loss network on the CPU side: utils.parse_layers, the Torch7 loss-network reader (trimming, cudnn.* and
-SpatialConvolutionMM names, 2-D weights, ceil_mode, refusals) and the CPU emulation of the N-block convolution plan that runs
+SpatialConvolutionMM names, 2-D weights, ceil_mode, refusals), fav_percep_create's refusal of geometries the planner cannot
+run, and the CPU emulation of the N-block convolution plan that runs
 VGG-16's 256- and 512-channel layers (tests/emu/nblock_emu.cu)."""
 import ctypes as C
 import os
@@ -98,6 +99,28 @@ def test_vgg16_shapes_and_default_layers():
     assert convs[:10] == [(3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256), (256, 256), (256, 512), (512, 512), (512, 512)]
 
 
+def _conv(cin, cout, k, stride=1, pad=None):
+    return dict(type="conv", cin=cin, cout=cout, k=k, stride=stride, pad=k // 2 if pad is None else pad,
+                weight=np.zeros((cout, cin, k, k), np.float32), bias=np.zeros(cout, np.float32))
+
+
+@pytest.mark.parametrize("mods,module", [
+    ([_conv(3, 128, 3), dict(type="relu"), _conv(128, 64, 7)], 3),  # 7 filter rows x 4 channel groups = 28 K groups > 16
+    ([_conv(3, 16, 3), dict(type="relu"), _conv(16, 32, 5, stride=2)], 3),  # stride 2 is planned for k3 pad 1 only
+    ([_conv(3, 24, 3), dict(type="relu"), _conv(24, 32, 3)], 3),  # Cin must be <= 8 or a multiple of 16
+    ([_conv(3, 16, 3, stride=2)], 1),  # the parity-split operand needs Cin >= 16
+    ([_conv(3, 8, 3), dict(type="relu"), _conv(8, 16, 3, stride=2)], 3),
+])
+def test_unplannable_convolutions_are_refused_at_create(mods, module):
+    """A loss network the tensor-core planner cannot run fails in fav_percep_create, before any weights reach the GPU,
+    with FAV_ERR_UNSUPPORTED and the module's index."""
+    from fav_b200 import _lib, percep
+
+    with pytest.raises(_lib.FavError) as e:
+        percep.PerceptualCriterion(mods, [len(mods)], [1.0], [], [])
+    assert e.value.status == _lib.FAV_ERR_UNSUPPORTED and f"module {module}" in str(e.value), str(e.value)
+
+
 @pytest.fixture(scope="module")
 def nblock_emu():
     so = os.path.join(EMU, "libfav_emu_nblock.so")
@@ -117,6 +140,11 @@ def nblock_emu():
     (256, 512, 3, 1, 3, 7),    # conv4_1: 4 N blocks, 8 K groups
     (128, 256, 3, 1, 2, 130),  # conv3_1: 2 N blocks, two tiles per row
     (64, 200, 3, 1, 2, 5),     # a partial last N block (72 channels, N = 80)
+    # k >= 5, pad (k-1)/2 and Cout <= 4 (or a last N block that narrow): the stylization net's x-fold plan writes the final
+    # tanh image, so a loss-network conv of that shape must get the generic plan
+    (16, 3, 5, 2, 3, 9),
+    (64, 130, 5, 2, 3, 9),     # last N block of 2 channels
+    (32, 4, 7, 3, 2, 140),
 ])
 def test_emulated_nblock_plan_matches_direct_conv(nblock_emu, case):
     cin, cout, k, pad, H, W = case
