@@ -83,8 +83,11 @@ struct ConvJob {
   // timing ablations (env FAV_DBG, diagnostics only; results are wrong when non-zero): 1 = no epilogue stores/stats,
   // 2 = 16-byte weight copies, 4 = 16-byte patch copies, 8 = no epilogue at all
   int dbg;
-  // fused InstanceNorm statistics: per-channel sum / sum of squares of the stored values (double, atomics), or null
+  // fused InstanceNorm statistics: per-channel sum / sum of squares of the stored values (double, atomics), or null.
+  // Channel c of this job adds into stats[c] and stats[stats_pitch + c]: stats_pitch is the whole tensor's channel count, so
+  // the N blocks of a wide convolution fill disjoint slots of one [sum][sum of squares] array (conv_nblock_stats)
   double *stats;
+  int stats_pitch;
   // output placement: raw(y*oy_mul + oy_off, x*ox_mul + ox_off)
   float *raw;
   int raw_Cq, raw_Wp;

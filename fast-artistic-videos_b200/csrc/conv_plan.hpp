@@ -56,6 +56,9 @@ struct ConvDef {
   std::vector<ConvPhase> phases;
   ConvPhase fold;    // transposed conv: all 4 phases in one tcgen05 job (phase-fold); phases[] stay for the comparator
   bool has_fold = false;
+  // Cout > kMaxNBlock (stylization net): the ConvDef of each N block (plan_conv_nblocks); the tensor-core jobs come from
+  // these, the CUDA-core comparator keeps the whole convolution's phases.  Empty: one job per phase of this ConvDef.
+  std::vector<ConvDef> nblock;
   float *d_bias = nullptr;
   int pw = -1, pb = -1;  // param indices
 };
@@ -344,25 +347,57 @@ static inline void init_conv_def(ConvDef &c, const std::string &name, int cin, i
   c.out_mul = tr ? stride : 1;
 }
 
-// ---- N blocks: a plain convolution with Cout > kMaxNBlock runs as ceil(Cout / 128) jobs of <= 128 output channels each.
-// Block b is an ordinary convolution over every input channel with output channels [128 b, 128 b + cout_b): its own
-// ConvDef (so its own tables and packed weights), a bias slice, and a raw output pointer advanced by 128 b channels
-// (32 b channel quads of the [Ho][Cq][Wp][4] layout; the row pitch Cq stays the full tensor's).
+// ---- N blocks: a convolution with Cout > kMaxNBlock runs as ceil(Cout / 128) jobs of <= 128 output channels each (per
+// sub-pixel phase, for a transposed convolution).  Block b is an ordinary convolution over every input channel with output
+// channels [128 b, 128 b + cout_b): its own ConvDef (so its own tables and packed weights), a bias slice, a raw output
+// pointer advanced by 128 b channels (32 b channel quads of the [Ho][Cq][Wp][4] layout; the row pitch Cq stays the full
+// tensor's) and, in the stylization net, the fused InstanceNorm statistics of those channels (conv_nblock_stats).
 static inline int conv_nblocks(int cout) { return (cout + kMaxNBlock - 1) / kMaxNBlock; }
 static inline int conv_nblock_cout(int cout, int b) { return std::min(kMaxNBlock, cout - b * kMaxNBlock); }
-// weights [Cout][Cin][k][k] -> the [cout_b][Cin][k][k] slice of block b
-static inline std::vector<float> conv_nblock_weights(const std::vector<float> &w, int cin, int cout, int k, int b) {
-  const size_t per = (size_t)cin * k * k;
-  const size_t c0 = (size_t)b * kMaxNBlock, n = (size_t)conv_nblock_cout(cout, b);
-  return std::vector<float>(w.begin() + c0 * per, w.begin() + (c0 + n) * per);
+// weights [Cout][Cin][k][k] -> the [cout_b][Cin][k][k] slice of block b; transposed weights [Cin][Cout][k][k] (Torch's
+// SpatialFullConvolution layout) -> the [Cin][cout_b][k][k] slice
+static inline std::vector<float> conv_nblock_weights(const std::vector<float> &w, int cin, int cout, int k, int b,
+                                                     bool transposed = false) {
+  const size_t kk = (size_t)k * k, c0 = (size_t)b * kMaxNBlock, n = (size_t)conv_nblock_cout(cout, b);
+  if (!transposed) return std::vector<float>(w.begin() + c0 * cin * kk, w.begin() + (c0 + n) * cin * kk);
+  std::vector<float> s;
+  s.reserve((size_t)cin * n * kk);
+  for (int ci = 0; ci < cin; ++ci) {
+    const auto first = w.begin() + ((size_t)ci * cout + c0) * kk;
+    s.insert(s.end(), first, first + n * kk);
+  }
+  return s;
 }
-// the ConvDef of N block b of a loss-network convolution (raw output, so never the x-fold plan)
-static inline void init_nblock_conv_def(ConvDef &c, const std::string &name, int cin, int cout, int k, int stride, int pad, int b) {
-  init_conv_def(c, name, cin, conv_nblock_cout(cout, b), k, stride, pad, false, 0);
+// the ConvDef of N block b (raw output, so never the x-fold plan)
+static inline void init_nblock_conv_def(ConvDef &c, const std::string &name, int cin, int cout, int k, int stride, int pad, int b,
+                                        bool transposed = false, int adj = 0) {
+  init_conv_def(c, name, cin, conv_nblock_cout(cout, b), k, stride, pad, transposed, adj);
   c.raw_out = true;
   build_phases(c);
 }
 static inline int64_t conv_nblock_raw_offset(int b, int raw_Wp) { return (int64_t)b * (kMaxNBlock / 4) * raw_Wp * 4; }
+// fused InstanceNorm statistics of block b: sums = the whole tensor's [sum][sum of squares] array of cout channels each; the
+// epilogue adds channel c of the block into job.stats[c] and job.stats[job.stats_pitch + c]
+static inline void conv_nblock_stats(ConvJob &j, double *sums, int cout, int b) {
+  j.stats = sums ? sums + (int64_t)b * kMaxNBlock : nullptr;
+  j.stats_pitch = cout;
+}
+// K-step tables of every phase of a stylization-net convolution, or of every N block's phases when Cout > kMaxNBlock.  A
+// geometry the tensor-core planner cannot run fails here with FAV_ERR_UNSUPPORTED and the layer's name.
+static inline int plan_conv_nblocks(ConvDef &c) {
+  c.nblock.clear();
+  if (conv_nblocks(c.cout) == 1) {
+    for (ConvPhase &ph : c.phases) FAV_TRY(build_phase_tables(c, ph));
+    return FAV_OK;
+  }
+  for (int b = 0; b < conv_nblocks(c.cout); ++b) {
+    ConvDef cb;
+    init_nblock_conv_def(cb, c.name, c.cin, c.cout, c.k, c.stride, c.pad, b, c.transposed, c.adj);
+    for (ConvPhase &ph : cb.phases) FAV_TRY(build_phase_tables(cb, ph));
+    c.nblock.push_back(std::move(cb));
+  }
+  return FAV_OK;
+}
 
 // packed tcgen05 weights of one phase: [group][chunk][hi|lo][step][k8 half][Npad][8] fp16 (as uint16 bit patterns)
 static inline std::vector<uint16_t> pack_phase_weights(const ConvDef &c, const ConvPhase &ph, const std::vector<float> &w) {

@@ -216,7 +216,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
 #pragma unroll
       for (int w = 0; w < 8; ++w) { ssum += slot[w * 256 + ch]; qsum += slot[w * 256 + 128 + ch]; }
       atomicAdd(job.stats + ch, (double)ssum);
-      atomicAdd(job.stats + job.Cout + ch, (double)qsum);
+      atomicAdd(job.stats + job.stats_pitch + ch, (double)qsum);
     }
   }
 }

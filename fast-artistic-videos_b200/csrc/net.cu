@@ -170,13 +170,30 @@ static int dev_upload(fav_net *net, const std::vector<T> &h, T **out) {
   return FAV_OK;
 }
 
+// packed tensor-core weights of every phase of c (K-step tables from plan_conv_nblocks)
+static int pack_tc_weights(fav_net *net, ConvDef &c, const std::vector<float> &w) {
+  for (auto &ph : c.phases) {
+    std::vector<uint16_t> pk = pack_phase_weights(c, ph, w);
+    uint16_t *d = nullptr;
+    FAV_TRY(dev_upload(net, pk, &d));
+    ph.d_b_tc = reinterpret_cast<uint4 *>(d);
+  }
+  return FAV_OK;
+}
+
 static int pack_conv_weights(fav_net *net, ConvDef &c) {
   const std::vector<float> &w = net->params[c.pw].host;
   std::vector<float> bias(c.Npad, 0.f);
   for (int i = 0; i < c.cout; ++i) bias[i] = net->params[c.pb].host[i];
   FAV_TRY(dev_upload(net, bias, &c.d_bias));
+  for (size_t b = 0; b < c.nblock.size(); ++b) {  // N blocks: weight and bias slices
+    ConvDef &cb = c.nblock[b];
+    std::vector<float> bb(cb.Npad, 0.f);
+    for (int i = 0; i < cb.cout; ++i) bb[i] = bias[b * kMaxNBlock + i];
+    FAV_TRY(dev_upload(net, bb, &cb.d_bias));
+    FAV_TRY(pack_tc_weights(net, cb, conv_nblock_weights(w, c.cin, c.cout, c.k, (int)b, c.transposed)));
+  }
   for (auto &ph : c.phases) {
-    FAV_TRY(build_phase_tables(c, ph));
     // CUDA-core comparator layout: [tap][Cin_pad][Cout_pad8]
     std::vector<float> ws((size_t)ph.taps.size() * c.cin_pad * c.cout_pad8, 0.f);
     for (size_t t = 0; t < ph.taps.size(); ++t)
@@ -184,11 +201,8 @@ static int pack_conv_weights(fav_net *net, ConvDef &c) {
         for (int co = 0; co < c.cout; ++co)
           ws[(t * c.cin_pad + ci) * c.cout_pad8 + co] = weight_at(c, w, co, ci, ph.taps[t].ky, ph.taps[t].kx);
     FAV_TRY(dev_upload(net, ws, &ph.d_w_simt));
-    std::vector<uint16_t> pk = pack_phase_weights(c, ph, w);
-    uint16_t *d = nullptr;
-    FAV_TRY(dev_upload(net, pk, &d));
-    ph.d_b_tc = reinterpret_cast<uint4 *>(d);
   }
+  if (c.nblock.empty()) FAV_TRY(pack_tc_weights(net, c, w));
   if (c.has_fold) {  // transposed conv: one tcgen05 job for all four sub-pixel phases
     std::vector<uint16_t> pk = pack_phase_fold(c, c.fold, w);
     uint16_t *d = nullptr;
@@ -215,39 +229,48 @@ static int make_operand(Plan &pl, int C, int H, int W, const ConvDef *consumer, 
   return FAV_OK;
 }
 
-static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &c, bool last, float *out3) {
+// tensor-core jobs of c (one per phase, per N block when Cout > kMaxNBlock) and CUDA-core comparator jobs (one per phase);
+// stats: the [sum][sum of squares] slots of c's output for the fused InstanceNorm statistics, or null
+static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &c, bool last, float *out3, double *stats) {
   const Operand &in = pl.ops[st.src];
-  bool fold_done = false;
-  for (const ConvPhase &ph0 : c.phases) {
-    const bool use_fold = c.has_fold && !getenv("FAV_NO_FOLD");
-    const ConvPhase &ph = ph0;
-    ConvJob j;
-    if (use_fold) {
-      if (!fold_done) {
-        FAV_TRY(fill_conv_job(c, c.fold, in, j));
-        j.b = c.fold.d_b_tc; j.bias = c.d_bias;
-        j.raw = st.raw.p; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
-        j.final_mode = 0; j.out3 = out3; j.tanh_c = net->tanh_c;
+  const int nb = c.nblock.empty() ? 1 : (int)c.nblock.size();
+  for (int b = 0; b < nb; ++b) {
+    const ConvDef &cd = c.nblock.empty() ? c : c.nblock[b];
+    float *raw = st.raw.p + conv_nblock_raw_offset(b, st.raw.Wp);
+    bool fold_done = false;
+    for (const ConvPhase &ph : cd.phases) {
+      const bool use_fold = cd.has_fold && !getenv("FAV_NO_FOLD");
+      ConvJob j;
+      if (use_fold) {
+        if (!fold_done) {
+          FAV_TRY(fill_conv_job(cd, cd.fold, in, j));
+          j.b = cd.fold.d_b_tc; j.bias = cd.d_bias;
+          j.raw = raw; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
+          j.final_mode = 0; j.out3 = out3; j.tanh_c = net->tanh_c;
+          conv_nblock_stats(j, stats, c.cout, b);
+          conv_tc_choose_slots(j);
+          if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
+          if (conv_tc_smem_bytes(j) > 227 * 1024) { set_error("conv %s: shared memory budget exceeded (fold)", c.name.c_str()); return FAV_ERR_UNSUPPORTED; }
+          st.tc.push_back(j);
+          fold_done = true;
+        }
+      } else {
+        FAV_TRY(fill_conv_job(cd, ph, in, j));
+        j.b = ph.d_b_tc; j.bias = cd.d_bias;
+        j.raw = raw; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
+        j.final_mode = last ? 1 : 0; j.out3 = out3; j.tanh_c = net->tanh_c;
+        conv_nblock_stats(j, stats, c.cout, b);
         conv_tc_choose_slots(j);
         if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
-        if (conv_tc_smem_bytes(j) > 227 * 1024) { set_error("conv %s: shared memory budget exceeded (fold)", c.name.c_str()); return FAV_ERR_UNSUPPORTED; }
+        if (conv_tc_smem_bytes(j) > 227 * 1024) {
+          set_error("conv %s: shared memory budget exceeded", c.name.c_str());
+          return FAV_ERR_UNSUPPORTED;
+        }
         st.tc.push_back(j);
-        fold_done = true;
       }
-    } else {
-    FAV_TRY(fill_conv_job(c, ph, in, j));
-    j.b = ph.d_b_tc; j.bias = c.d_bias;
-    j.raw = st.raw.p; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
-    j.final_mode = last ? 1 : 0; j.out3 = out3; j.tanh_c = net->tanh_c;
-    conv_tc_choose_slots(j);
-    if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
-    if (conv_tc_smem_bytes(j) > 227 * 1024) {
-      set_error("conv %s: shared memory budget exceeded", c.name.c_str());
-      return FAV_ERR_UNSUPPORTED;
     }
-    st.tc.push_back(j);
-    }
-
+  }
+  for (const ConvPhase &ph : c.phases) {
     SimtJob s;
     memset(&s, 0, sizeof(s));
     s.in = in; s.sy = s.sx = c.in_stride; s.ntaps = (int)ph.taps.size();
@@ -338,15 +361,19 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       cs.raw.p = (pos & 1) ? pl->raw_buf2 : pl->raw_buf; cs.raw.C = c.cout; cs.raw.Cq = round_up(c.cout, 4) / 4; cs.raw.H = ho; cs.raw.W = wo;
       cs.raw.Hp = ho + 2; cs.raw.Wp = round_up(wo, kTileM);
       const bool last = op.last && i == n - 1;
-      FAV_TRY(build_conv_jobs(net, *pl, cs, c, last, nullptr));
-      // second conv of a residual block: fold the preceding InstanceNorm + ReLU pass into its patch producers
+      // statistics fused into the epilogue: every conv but the last is followed by InstanceNorm (checked below)
+      FAV_TRY(build_conv_jobs(net, *pl, cs, c, last, nullptr, last ? nullptr : pl->stats + stats_off));
+      // second conv of a residual block: fold the preceding InstanceNorm + ReLU pass into its patch producers.  Each N block
+      // of a wide conv normalises the whole patch on load itself (the A-side work is repeated per block); the per-channel
+      // tables hold at most 256 channels (conv_tc.cu kNlMaxC), wider blocks keep the separate in_apply pass.
       if (op.kind == 1 && i == 1 && !pl->steps.empty() && pl->steps.back().kind == 1 && !getenv("FAV_NO_NL")) {
         PlanStep &ap = pl->steps.back();
         const InDef &n = net->inorms[ap.inorm];
         const Operand &in = pl->ops[cs.src];
-        bool ok = ap.skip < 0 && n.C <= 256 && cs.tc.size() == 1;
-        if (ok) {
-          ConvJob &j = cs.tc[0];
+        bool ok = ap.skip < 0 && n.C <= 256;
+        std::vector<ConvJob> fused;
+        for (size_t k = 0; ok && k < cs.tc.size(); ++k) {
+          const ConvJob &j = cs.tc[k];
           ok = !j.rf_R && !j.pf && !j.xfold_kw && j.nseg == 1 && j.seg_dst16[0] == 0 && j.seg_len16[0] == j.pslab16 && j.row_mul == 1;
           if (ok) {
             ConvJob t = j;
@@ -356,9 +383,11 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
             t.nl_sums = pl->stats + ap.stats_off; t.nl_gamma = n.d_gamma; t.nl_beta = n.d_beta;
             t.nl_inv_count = 1.0 / ((double)ap.raw.H * ap.raw.W); t.nl_eps = 1e-5;
             conv_tc_choose_slots(t);
-            if (conv_tc_smem_bytes(t) <= 227 * 1024 && (t.b_resident || t.b_slots >= 2)) { j = t; ap.fused_nl = true; }
+            ok = conv_tc_smem_bytes(t) <= 227 * 1024 && (t.b_resident || t.b_slots >= 2);
+            fused.push_back(t);
           }
         }
+        if (ok && !fused.empty()) { cs.tc = std::move(fused); ap.fused_nl = true; }
       }
       if (last) { cs.layer_index = (int)oi; pl->steps.push_back(std::move(cs)); break; }
       RawTensor raw = cs.raw;
@@ -371,7 +400,6 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       }
       PlanStep ns;
       ns.kind = 1; ns.inorm = op.inorm[i]; ns.raw = raw; ns.stats_off = stats_off;
-      for (ConvJob &j : pl->steps.back().tc) j.stats = pl->stats + stats_off;  // statistics fused into the epilogue
       stats_off += 2 * c.cout;
       const ConvDef *consumer = pos + 1 < order.size() ? &net->convs[order[pos + 1]] : nullptr;
       FAV_TRY(make_operand(*pl, c.cout, ho, wo, consumer, &ns.dst));
@@ -661,6 +689,9 @@ int fav_net_finalize(fav_net_t *net) {
   FAV_REQUIRE(net, "fav_net_finalize: null net");
   if (net->finalized) return FAV_OK;
   for (Param &p : net->params) FAV_REQUIRE(p.set, "fav_net_finalize: parameter %s was never set", p.name.c_str());
+  // K-step tables (N blocks for Cout > 128) of every convolution, before any device work: a layer the tensor-core path
+  // cannot run is refused here, by name, rather than at the first forward
+  for (ConvDef &c : net->convs) FAV_TRY(plan_conv_nblocks(c));
   FAV_TRY(require_device());
   cudaDeviceProp prop;
   FAV_TRY(check_cuda(cudaGetDevice(&net->device), "cudaGetDevice"));
