@@ -96,7 +96,28 @@ struct ConvJob {
   int final_mode;  // 0 = raw, 1 = net space, 2 = fused vgg.deprocess
   float *out3;
   float tanh_c;
+  // operand epilogue (batch-normalized nets; set_opnd_epilogue): instead of the raw output, acc * epi_scale + bias (+ReLU)
+  // (+ the skip operand read at (y + epi_shave, x + epi_shave)) is split into fp16 hi / lo and stored at output (yo, xo),
+  // channel epi_c0 + c of epi_dst, the next convolution's operand.  epi_c0: the N block's first channel.
+  int opnd, epi_relu, epi_skip, epi_shave, epi_c0;
+  const float *epi_scale;
+  Operand epi_dst, epi_skip_op;
 };
+
+// Operand epilogue addressing, shared by conv_tc_kernel and its CPU emulator (tests/emu/opnd_epi_emu.cu).  Consumer thread t
+// (0..255) of a tile holds, for i < Npad / 8 and h < 2, the accumulator pair of channels c, c + 1 (c = 8i + 2 (t % 4)) of tile
+// pixel r0 + 8h (r0 = 64 (t / 128) + 16 (t / 32 % 4) + t % 32 / 4).  Returns false when that pair lies outside the job's
+// output (no store); else the 4-byte offsets of its fp16 pair in the hi / lo planes of epi_dst and, for a residual skip, of
+// epi_skip_op.
+__host__ __device__ inline bool opnd_epi_addr(const ConvJob &j, int tile, int t, int i, int h, int64_t &dst4, int64_t &skip4) {
+  const int y = tile / j.tiles_x, x = (tile - y * j.tiles_x) * j.tile_dx + (t >> 7) * 64 + ((t >> 5) & 3) * 16 + ((t & 31) >> 2) + 8 * h;
+  const int c = 8 * i + 2 * (t & 3);
+  if (x >= j.Wo || y >= j.Ho || c >= j.Cout) return false;
+  const int yo = y * j.oy_mul + j.oy_off, xo = x * j.ox_mul + j.ox_off;
+  dst4 = j.epi_dst.pair_off4(yo, xo, j.epi_c0 + c);
+  skip4 = j.epi_skip ? j.epi_skip_op.pair_off4(yo + j.epi_shave, xo + j.epi_shave, j.epi_c0 + c) : 0;
+  return true;
+}
 
 // CUDA-core comparator job (debug / bring-up path; same inputs and outputs as ConvJob)
 struct SimtJob {
@@ -128,10 +149,12 @@ void conv_tc_choose_slots(ConvJob &job);  // fills b_slots / b_resident from the
 // elementwise / reduction kernels of the net (net_kernels.cu)
 int launch_pack_input(const float *in, int Cin, int H, int W, int reflect, const Operand &dst, cudaStream_t st);
 int launch_in_stats(const RawTensor &raw, double *sums /*[2*C]*/, cudaStream_t st);
+// sums == null: no normalisation (batch-normalized nets on the CUDA-core comparator: ReLU / skip / pack only)
 int launch_in_apply(const RawTensor &raw, const double *sums, const float *gamma, const float *beta, float eps, int relu,
                     const Operand *skip, int shave, const Operand &dst, cudaStream_t st);
+// tab_mean / tab_scale non-null: a fixed per-channel affine (inference-mode BatchNorm) instead of the statistics of src
 int launch_up_in(const Operand &src, double *sums, const float *gamma, const float *beta, float eps, int relu, int scale,
-                 const Operand &dst, cudaStream_t st);
+                 const Operand &dst, cudaStream_t st, const float *tab_mean = nullptr, const float *tab_scale = nullptr);
 int launch_unpack_operand(const Operand &src, float *out_nchw, cudaStream_t st);
 
 }  // namespace fav

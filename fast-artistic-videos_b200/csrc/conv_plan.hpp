@@ -60,6 +60,7 @@ struct ConvDef {
   // these, the CUDA-core comparator keeps the whole convolution's phases.  Empty: one job per phase of this ConvDef.
   std::vector<ConvDef> nblock;
   float *d_bias = nullptr;
+  float *d_scale = nullptr;  // batch-normalized nets: the per-channel BN scale the operand epilogue applies (Npad floats)
   int pw = -1, pb = -1;  // param indices
 };
 
@@ -381,6 +382,15 @@ static inline int64_t conv_nblock_raw_offset(int b, int raw_Wp) { return (int64_
 static inline void conv_nblock_stats(ConvJob &j, double *sums, int cout, int b) {
   j.stats = sums ? sums + (int64_t)b * kMaxNBlock : nullptr;
   j.stats_pitch = cout;
+}
+// operand epilogue of a batch-normalized net's non-final convolution: job j of N block b writes acc * scale + bias (+ReLU)
+// (+skip: the block input `skip` shifted by `shave`) straight into `dst`, the next convolution's operand (opnd_epi_addr,
+// conv.cuh).  scale: the block's per-channel BN scale, bias the folded bias.  No raw output, no statistics.
+static inline void set_opnd_epilogue(ConvJob &j, int b, const float *scale, const Operand &dst, int relu, const Operand *skip,
+                                     int shave) {
+  j.opnd = 1; j.epi_scale = scale; j.epi_c0 = b * kMaxNBlock; j.epi_dst = dst; j.epi_relu = relu;
+  j.epi_skip = skip ? 1 : 0; j.epi_skip_op = skip ? *skip : Operand(); j.epi_shave = skip ? shave : 0;
+  j.raw = nullptr; j.stats = nullptr;
 }
 // K-step tables of every phase of a stylization-net convolution, or of every N block's phases when Cout > kMaxNBlock.  A
 // geometry the tensor-core planner cannot run fails here with FAV_ERR_UNSUPPORTED and the layer's name.

@@ -64,8 +64,10 @@ __device__ __forceinline__ void trace_put(const ConvJob &job, int word, long lon
   if (job.trace) job.trace[(size_t)blockIdx.x * kTraceWords + word] = (unsigned long long)v;
 }
 
-// consumer warpgroup: MMAs of one 64-pixel half of every tile of this CTA, then its epilogue
-template <int NT>
+// consumer warpgroup: MMAs of one 64-pixel half of every tile of this CTA, then its epilogue.
+// OPND: operand epilogue of batch-normalized nets (ConvJob::opnd) -- a template parameter, so the raw-output instances keep
+// their code and registers.
+template <int NT, bool OPND>
 __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, uint8_t *b_base, TcShared *sh, float *exch) {
   constexpr int NJ = NT / 8;
   const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -175,6 +177,35 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
         }
       continue;
     }
+    if constexpr (OPND) {
+      // the two channels c, c + 1 of each of the thread's two pixels: BN scale and bias (+ReLU) (+skip) -> fp16 hi / lo pair, one 4-byte store
+      // per plane; the 4 lanes of a quad fill one 16-byte (pixel, channel block) cell.  No statistics, no atomics.
+      uint32_t *dhi = reinterpret_cast<uint32_t *>(job.epi_dst.hi), *dlo = reinterpret_cast<uint32_t *>(job.epi_dst.lo);
+#pragma unroll
+      for (int i = 0; i < NJ; ++i) {
+        const int c = 8 * i + q2;
+        // bias and scale are padded to Npad
+        const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c)), s = __ldg(reinterpret_cast<const float2 *>(job.epi_scale + c));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          int64_t o, so;
+          if (!opnd_epi_addr(job, tile, threadIdx.x, i, h, o, so)) continue;
+          float v0 = fmaf(acc[4 * i + 2 * h], s.x, b.x), v1 = fmaf(acc[4 * i + 2 * h + 1], s.y, b.y);
+          if (job.epi_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          if (job.epi_skip) {  // ConcatTable{conv_block, ShaveImage / Identity} -> CAddTable; same arithmetic as in_apply
+            const uint32_t sh = __ldg(reinterpret_cast<const uint32_t *>(job.epi_skip_op.hi) + so);
+            const uint32_t sl = __ldg(reinterpret_cast<const uint32_t *>(job.epi_skip_op.lo) + so);
+            const float2 fh = __half22float2(*reinterpret_cast<const __half2 *>(&sh));
+            const float2 fl = __half22float2(*reinterpret_cast<const __half2 *>(&sl));
+            v0 += fh.x + fl.x; v1 += fh.y + fl.y;
+          }
+          uint32_t hw, lw;
+          split_pair(v0, v1, hw, lw);
+          dhi[o] = hw; dlo[o] = lw;
+        }
+      }
+      continue;
+    }
     const bool stats = job.stats && !(job.dbg & 64);
 #pragma unroll
     for (int i = 0; i < NJ; ++i) {
@@ -221,7 +252,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   }
 }
 
-template <int NT>
+template <int NT, bool OPND>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ ConvJob job) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t a_stage_bytes = (uint32_t)job.stage16 * 16u;  // one of hi / lo
@@ -261,7 +292,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   const int ngroups = job.ngroups, nchunks = job.nchunks;
 
   if (warp < 8) {
-    tc_consume<NT>(job, a_base, b_base, sh, exch);
+    tc_consume<NT, OPND>(job, a_base, b_base, sh, exch);
   } else if (job.nl && warp >= kAWarp) {
     // ===== norm-on-load patch producers: raw fp32 -> InstanceNorm (+ReLU) -> fp16 hi/lo -> MMA-ready stage =====
     // A warp owns whole (patch row, channel block) slabs: lanes run along x (coalesced 512-byte loads), up to
@@ -388,7 +419,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
 
 static size_t tc_fixed_smem(const ConvJob &job) {
   return (size_t)job.a_stages * 2 * job.stage16 * 16 + sizeof(TcShared) + 128 +
-         (job.xfold_kw ? (size_t)kTileM * kExchPitch * 4 : (size_t)(256 + 8 * 2 * 128) * 4) + (job.nl ? (size_t)3 * kNlMaxC * 4 : 0);
+         (job.xfold_kw ? (size_t)kTileM * kExchPitch * 4 : job.opnd ? 0 : (size_t)(256 + 8 * 2 * 128) * 4) +
+         (job.nl ? (size_t)3 * kNlMaxC * 4 : 0);
 }
 size_t conv_tc_smem_bytes(const ConvJob &job) { return tc_fixed_smem(job) + (size_t)job.b_slots * job.chunk16 * 16; }
 
@@ -441,19 +473,15 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
     return FAV_ERR_UNSUPPORTED;
   }
   void (*kernel)(ConvJob) = nullptr;
+#define FAV_TC_CASE(N) case N: kernel = job.opnd ? conv_tc_kernel<N, true> : conv_tc_kernel<N, false>; break;
   switch (job.Npad) {
-    case 16: kernel = conv_tc_kernel<16>; break;
-    case 32: kernel = conv_tc_kernel<32>; break;
-    case 48: kernel = conv_tc_kernel<48>; break;
-    case 64: kernel = conv_tc_kernel<64>; break;
-    case 80: kernel = conv_tc_kernel<80>; break;
-    case 96: kernel = conv_tc_kernel<96>; break;
-    case 112: kernel = conv_tc_kernel<112>; break;
-    case 128: kernel = conv_tc_kernel<128>; break;
+    FAV_TC_CASE(16) FAV_TC_CASE(32) FAV_TC_CASE(48) FAV_TC_CASE(64) FAV_TC_CASE(80) FAV_TC_CASE(96) FAV_TC_CASE(112)
+    FAV_TC_CASE(128)
     default:
       set_error("conv_tc: no wgmma kernel for N = %d (multiples of 16 up to 128)", job.Npad);
       return FAV_ERR_UNSUPPORTED;
   }
+#undef FAV_TC_CASE
   job.trace = conv_trace_claim((size_t)(job.ntiles < num_sms ? job.ntiles : num_sms) * kTraceWords);
   size_t smem = conv_tc_smem_bytes(job);
   if (smem > 227 * 1024) {
@@ -461,11 +489,11 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
     return FAV_ERR_UNSUPPORTED;
   }
   // the opt-in to > 48 KB of dynamic shared memory is a PER-DEVICE attribute of each instantiation
-  static std::atomic<uint64_t> attr_set[9];
+  static std::atomic<uint64_t> attr_set[18];
   int dev = 0;
   FAV_TRY(check_cuda(cudaGetDevice(&dev), "cudaGetDevice"));
   const uint64_t bit = 1ull << (dev & 63);
-  std::atomic<uint64_t> &set = attr_set[job.Npad / 16];
+  std::atomic<uint64_t> &set = attr_set[job.Npad / 16 + (job.opnd ? 9 : 0)];
   if (!(set.load(std::memory_order_acquire) & bit)) {
     FAV_TRY(check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
                        "cudaFuncSetAttribute(conv_tc)"));

@@ -38,11 +38,17 @@ struct Param {
   bool set = false;
 };
 
+// a normalisation layer: InstanceNormalization, or (batch-normalized nets) inference-mode SpatialBatchNormalization
 struct InDef {
   std::string name;
   int C = 0;
   float *d_gamma = nullptr, *d_beta = nullptr;
   int pw = -1, pb = -1;
+  // batch norm: running statistics and eps; conv = the convolution it directly follows (folded into it at finalize,
+  // fold_batch_norms), -1 after a UX upsampling (applied as the fixed per-channel affine d_mean / d_scale by up_apply)
+  int pm = -1, pv = -1, pe = -1, conv = -1;
+  std::vector<float> h_mean, h_scale;
+  float *d_mean = nullptr, *d_scale = nullptr;
 };
 
 // arch-level program
@@ -68,6 +74,7 @@ struct PlanStep {
   std::vector<ConvJob> tc;
   std::vector<SimtJob> simt;
   int stats_off = 0;
+  int raw_sel = 0;       // raw.p is Plan::raw_buf (0) or raw_buf2 (1)
   int layer_index = -1;  // arch token index whose output this step completes (for fav_net_layer_output)
   bool fused_nl = false; // kind 1: the tcgen05 consumer normalises on load (conv_tc.cu), this pass is skipped
 };
@@ -77,6 +84,7 @@ struct Plan {
   std::vector<Operand> ops;
   std::vector<void *> allocs;
   float *raw_buf = nullptr, *raw_buf2 = nullptr;  // consecutive convolutions alternate (norm-on-load reads one, writes the other)
+  size_t raw_bytes = 0;  // of each; a batch-normalized net allocates them only for the CUDA-core comparator (ensure_raw)
   double *stats = nullptr;
   size_t stats_bytes = 0;
   float *msb = nullptr;
@@ -106,6 +114,7 @@ struct fav_net {
   float tanh_c = 150.f;
   int in_dim = 7;
   int reflect_pad = 0;
+  bool bn = false;  // use_instance_norm = 0: SpatialBatchNormalization in evaluate mode (models_video.lua:21-25,33-37,121-127)
   std::vector<Param> params;
   std::vector<ConvDef> convs;
   std::vector<InDef> inorms;
@@ -151,11 +160,17 @@ static int add_conv(fav_net *net, const std::string &name, int cin, int cout, in
   net->convs.push_back(std::move(c));
   return (int)net->convs.size() - 1;
 }
-static int add_in(fav_net *net, const std::string &name, int C) {
+static int add_in(fav_net *net, const std::string &name, int C, int conv) {
   InDef n;
   n.name = name; n.C = C;
   n.pw = add_param(net, name + ".weight", {C});
   n.pb = add_param(net, name + ".bias", {C});
+  if (net->bn) {
+    n.pm = add_param(net, name + ".running_mean", {C});
+    n.pv = add_param(net, name + ".running_var", {C});
+    n.pe = add_param(net, name + ".eps", {1});
+    n.conv = conv;
+  }
   net->inorms.push_back(std::move(n));
   return (int)net->inorms.size() - 1;
 }
@@ -181,16 +196,21 @@ static int pack_tc_weights(fav_net *net, ConvDef &c, const std::vector<float> &w
   return FAV_OK;
 }
 
-static int pack_conv_weights(fav_net *net, ConvDef &c) {
-  const std::vector<float> &w = net->params[c.pw].host;
-  std::vector<float> bias(c.Npad, 0.f);
-  for (int i = 0; i < c.cout; ++i) bias[i] = net->params[c.pb].host[i];
+// w: the weights the tensor cores multiply with, b the bias; w_simt: the CUDA-core comparator's weights; scale: empty, or the
+// per-channel BatchNorm scale the operand epilogue applies (fold_batch_norms)
+static int pack_conv_weights(fav_net *net, ConvDef &c, const std::vector<float> &w, const std::vector<float> &b,
+                             const std::vector<float> &w_simt, const std::vector<float> &scale) {
+  std::vector<float> bias(c.Npad, 0.f), sc(c.Npad, 0.f);
+  for (int i = 0; i < c.cout; ++i) bias[i] = b[i];
+  for (size_t i = 0; i < scale.size(); ++i) sc[i] = scale[i];
   FAV_TRY(dev_upload(net, bias, &c.d_bias));
-  for (size_t b = 0; b < c.nblock.size(); ++b) {  // N blocks: weight and bias slices
+  if (!scale.empty()) FAV_TRY(dev_upload(net, sc, &c.d_scale));
+  for (size_t b = 0; b < c.nblock.size(); ++b) {  // N blocks: weight, bias and scale slices
     ConvDef &cb = c.nblock[b];
-    std::vector<float> bb(cb.Npad, 0.f);
-    for (int i = 0; i < cb.cout; ++i) bb[i] = bias[b * kMaxNBlock + i];
+    std::vector<float> bb(cb.Npad, 0.f), sb(cb.Npad, 0.f);
+    for (int i = 0; i < cb.cout; ++i) { bb[i] = bias[b * kMaxNBlock + i]; sb[i] = sc[b * kMaxNBlock + i]; }
     FAV_TRY(dev_upload(net, bb, &cb.d_bias));
+    if (!scale.empty()) FAV_TRY(dev_upload(net, sb, &cb.d_scale));
     FAV_TRY(pack_tc_weights(net, cb, conv_nblock_weights(w, c.cin, c.cout, c.k, (int)b, c.transposed)));
   }
   for (auto &ph : c.phases) {
@@ -199,7 +219,7 @@ static int pack_conv_weights(fav_net *net, ConvDef &c) {
     for (size_t t = 0; t < ph.taps.size(); ++t)
       for (int ci = 0; ci < c.cin; ++ci)
         for (int co = 0; co < c.cout; ++co)
-          ws[(t * c.cin_pad + ci) * c.cout_pad8 + co] = weight_at(c, w, co, ci, ph.taps[t].ky, ph.taps[t].kx);
+          ws[(t * c.cin_pad + ci) * c.cout_pad8 + co] = weight_at(c, w_simt, co, ci, ph.taps[t].ky, ph.taps[t].kx);
     FAV_TRY(dev_upload(net, ws, &ph.d_w_simt));
   }
   if (c.nblock.empty()) FAV_TRY(pack_tc_weights(net, c, w));
@@ -208,6 +228,52 @@ static int pack_conv_weights(fav_net *net, ConvDef &c) {
     uint16_t *d = nullptr;
     FAV_TRY(dev_upload(net, pk, &d));
     c.fold.d_b_tc = reinterpret_cast<uint4 *>(d);
+  }
+  return FAV_OK;
+}
+
+// The bias each convolution runs with, its folded weights and its per-channel scale.  A batch-normalized net folds every
+// inference-mode BatchNorm that directly follows a convolution into it, in double: s = weight / sqrt(running_var + eps),
+// W' = W s along the output channel (dimension 1 of a transposed conv's [Cin][Cout][k][k]), b' = (b - running_mean) s + bias.
+// The CUDA-core comparator multiplies with W' (fp32).  The tensor cores keep W and the operand epilogue computes acc s + b':
+// W' is often tiny (s ~ 1e-2 after a first conv whose input is in pixel units), and the lo half of its fp16 hi/lo split then
+// falls into the fp16 subnormals (DESIGN.md 4.1: folded weights put the net-space output 0.033 off the fp64 oracle).
+// The BN of a UX token comes after the upsampling, behind the previous layer's ReLU, so it is kept as the affine
+// (x - running_mean) s + bias (h_mean / h_scale).
+static int fold_batch_norms(fav_net *net, std::vector<std::vector<float>> &w, std::vector<std::vector<float>> &b,
+                            std::vector<std::vector<float>> &scale) {
+  w.resize(net->convs.size()); b.resize(net->convs.size()); scale.assign(net->convs.size(), {});
+  for (size_t i = 0; i < net->convs.size(); ++i) { w[i] = net->params[net->convs[i].pw].host; b[i] = net->params[net->convs[i].pb].host; }
+  if (!net->bn) return FAV_OK;
+  for (InDef &n : net->inorms) {
+    const std::vector<float> &g = net->params[n.pw].host, &be = net->params[n.pb].host, &m = net->params[n.pm].host,
+                             &v = net->params[n.pv].host;
+    const double eps = net->params[n.pe].host[0];
+    std::vector<double> sc(n.C);
+    for (int ch = 0; ch < n.C; ++ch) {
+      const double d = (double)v[ch] + eps;
+      if (!std::isfinite(d) || !(d > 0) || !std::isfinite(g[ch]) || !std::isfinite(be[ch]) || !std::isfinite(m[ch])) {
+        set_error("batch norm %s, channel %d: weight %g, bias %g, running_mean %g, running_var + eps %g (all must be finite, "
+                  "running_var + eps > 0)", n.name.c_str(), ch, g[ch], be[ch], m[ch], d);
+        return FAV_ERR_INVALID;
+      }
+      sc[ch] = (double)g[ch] / std::sqrt(d);
+    }
+    if (n.conv < 0) {
+      n.h_mean = m;
+      n.h_scale.resize(n.C);
+      for (int ch = 0; ch < n.C; ++ch) n.h_scale[ch] = (float)sc[ch];
+      continue;
+    }
+    const ConvDef &c = net->convs[n.conv];
+    const int64_t kk = (int64_t)c.k * c.k;
+    std::vector<float> &wc = w[n.conv], &bc = b[n.conv];
+    for (int64_t i = 0; i < (int64_t)wc.size(); ++i) {
+      const int co = (int)(c.transposed ? (i / kk) % c.cout : i / (kk * c.cin));
+      wc[i] = (float)((double)wc[i] * sc[co]);
+    }
+    for (int co = 0; co < c.cout; ++co) bc[co] = (float)(((double)bc[co] - m[co]) * sc[co] + be[co]);
+    scale[n.conv].assign(sc.begin(), sc.end());
   }
   return FAV_OK;
 }
@@ -230,8 +296,10 @@ static int make_operand(Plan &pl, int C, int H, int W, const ConvDef *consumer, 
 }
 
 // tensor-core jobs of c (one per phase, per N block when Cout > kMaxNBlock) and CUDA-core comparator jobs (one per phase);
-// stats: the [sum][sum of squares] slots of c's output for the fused InstanceNorm statistics, or null
-static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &c, bool last, float *out3, double *stats) {
+// stats: the [sum][sum of squares] slots of c's output for the fused InstanceNorm statistics, or null; epi (batch-normalized
+// nets): the operand step whose ReLU / skip / packing the tensor-core epilogue performs (set_opnd_epilogue), or null
+static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &c, bool last, float *out3, double *stats,
+                           const PlanStep *epi = nullptr) {
   const Operand &in = pl.ops[st.src];
   const int nb = c.nblock.empty() ? 1 : (int)c.nblock.size();
   for (int b = 0; b < nb; ++b) {
@@ -260,6 +328,8 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
         j.raw = raw; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
         j.final_mode = last ? 1 : 0; j.out3 = out3; j.tanh_c = net->tanh_c;
         conv_nblock_stats(j, stats, c.cout, b);
+        if (epi)
+          set_opnd_epilogue(j, b, cd.d_scale, pl.ops[epi->dst], epi->relu, epi->skip >= 0 ? &pl.ops[epi->skip] : nullptr, epi->shave);
         conv_tc_choose_slots(j);
         if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
         if (conv_tc_smem_bytes(j) > 227 * 1024) {
@@ -304,7 +374,7 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
   {
     int h = H + 2 * R, w = W + 2 * R;
     for (auto &op : net->ops) {
-      if (op.kind == 2) { h *= op.scale; w *= op.scale; stats_slots += 2 * net->inorms[op.inorm[0]].C; continue; }
+      if (op.kind == 2) { h *= op.scale; w *= op.scale; stats_slots += net->bn ? 0 : 2 * net->inorms[op.inorm[0]].C; continue; }
       int n = op.kind == 1 ? 2 : 1;
       for (int i = 0; i < n; ++i) {
         const ConvDef &c = net->convs[op.conv[i]];
@@ -312,12 +382,15 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
         conv_out_size(c, h, w, &ho, &wo);
         raw_max = std::max(raw_max, (size_t)(ho + 2) * round_up(c.cout, 4) * round_up(wo, kTileM));
         h = ho; w = wo;
-        if (op.inorm[i] >= 0) stats_slots += 2 * c.cout;
+        if (op.inorm[i] >= 0 && !net->bn) stats_slots += 2 * c.cout;
       }
     }
   }
-  FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf, raw_max * sizeof(float) + 4096));
-  FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf2, raw_max * sizeof(float) + 4096));
+  pl->raw_bytes = raw_max * sizeof(float) + 4096;
+  if (!net->bn) {  // a batch-normalized net's tensor-core epilogues write operands, not raw tensors
+    FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf, pl->raw_bytes));
+    FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf2, pl->raw_bytes));
+  }
   pl->stats_bytes = std::max(1, stats_slots) * sizeof(double);
   FAV_TRY(alloc_zero(*pl, (void **)&pl->stats, pl->stats_bytes));
   FAV_TRY(alloc_zero(*pl, (void **)&pl->msb, std::max(1, stats_slots) * 2 * sizeof(float)));
@@ -341,7 +414,7 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       PlanStep us;
       us.kind = 2; us.scale = op.scale; us.inorm = op.inorm[0]; us.src = cur; us.relu = 1; us.stats_off = stats_off;
       const int C = net->inorms[op.inorm[0]].C;
-      stats_off += 2 * C;
+      if (!net->bn) stats_off += 2 * C;
       const ConvDef *consumer = pos < order.size() ? &net->convs[order[pos]] : nullptr;
       FAV_TRY(make_operand(*pl, C, pl->ops[cur].H * op.scale, pl->ops[cur].W * op.scale, consumer, &us.dst));
       cur = us.dst;
@@ -358,15 +431,42 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       cs.kind = 0; cs.conv = op.conv[i]; cs.src = cur;
       int ho, wo;
       conv_out_size(c, pl->ops[cur].H, pl->ops[cur].W, &ho, &wo);
-      cs.raw.p = (pos & 1) ? pl->raw_buf2 : pl->raw_buf; cs.raw.C = c.cout; cs.raw.Cq = round_up(c.cout, 4) / 4; cs.raw.H = ho; cs.raw.W = wo;
+      cs.raw.p = (pos & 1) ? pl->raw_buf2 : pl->raw_buf; cs.raw_sel = (int)(pos & 1);
+      cs.raw.C = c.cout; cs.raw.Cq = round_up(c.cout, 4) / 4; cs.raw.H = ho; cs.raw.W = wo;
       cs.raw.Hp = ho + 2; cs.raw.Wp = round_up(wo, kTileM);
       const bool last = op.last && i == n - 1;
-      // statistics fused into the epilogue: every conv but the last is followed by InstanceNorm (checked below)
-      FAV_TRY(build_conv_jobs(net, *pl, cs, c, last, nullptr, last ? nullptr : pl->stats + stats_off));
+      if (last) {
+        FAV_TRY(build_conv_jobs(net, *pl, cs, c, true, nullptr, nullptr));
+        cs.layer_index = (int)oi;
+        pl->steps.push_back(std::move(cs));
+        break;
+      }
+      // InstanceNorm / BatchNorm (+ReLU) (+skip) -> operand for the next convolution
+      if (op.inorm[i] < 0 || c.cout % 8) {
+        set_error("layer %s: a non-final convolution must be followed by InstanceNormalization (Cout %% 8 == 0)",
+                  c.name.c_str());
+        return FAV_ERR_UNSUPPORTED;
+      }
+      PlanStep ns;
+      ns.kind = 1; ns.inorm = op.inorm[i]; ns.raw = cs.raw; ns.raw_sel = cs.raw_sel; ns.stats_off = stats_off;
+      if (!net->bn) stats_off += 2 * c.cout;
+      const ConvDef *consumer = pos + 1 < order.size() ? &net->convs[order[pos + 1]] : nullptr;
+      FAV_TRY(make_operand(*pl, c.cout, ho, wo, consumer, &ns.dst));
+      if (op.kind == 1) {
+        ns.relu = i == 0 ? 1 : (op.relu ? 1 : 0);               // CX: needs_relu after the block (models_video.lua:108)
+        ns.skip = (i == 1 && op.skip) ? block_in : -1;          // RX: ShaveImage(2) / Identity of the block input (:46-50)
+        ns.shave = op.shave;
+      } else {
+        ns.relu = op.relu ? 1 : 0;
+      }
+      // InstanceNorm: statistics fused into the epilogue.  BatchNorm (folded into the conv): the epilogue performs ns itself,
+      // which then only runs after the CUDA-core comparator
+      FAV_TRY(build_conv_jobs(net, *pl, cs, c, false, nullptr, net->bn ? nullptr : pl->stats + ns.stats_off,
+                              net->bn ? &ns : nullptr));
       // second conv of a residual block: fold the preceding InstanceNorm + ReLU pass into its patch producers.  Each N block
       // of a wide conv normalises the whole patch on load itself (the A-side work is repeated per block); the per-channel
       // tables hold at most 256 channels (conv_tc.cu kNlMaxC), wider blocks keep the separate in_apply pass.
-      if (op.kind == 1 && i == 1 && !pl->steps.empty() && pl->steps.back().kind == 1 && !getenv("FAV_NO_NL")) {
+      if (!net->bn && op.kind == 1 && i == 1 && !pl->steps.empty() && pl->steps.back().kind == 1 && !getenv("FAV_NO_NL")) {
         PlanStep &ap = pl->steps.back();
         const InDef &n = net->inorms[ap.inorm];
         const Operand &in = pl->ops[cs.src];
@@ -389,27 +489,7 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
         }
         if (ok && !fused.empty()) { cs.tc = std::move(fused); ap.fused_nl = true; }
       }
-      if (last) { cs.layer_index = (int)oi; pl->steps.push_back(std::move(cs)); break; }
-      RawTensor raw = cs.raw;
       pl->steps.push_back(std::move(cs));
-      // InstanceNorm (+ReLU) (+skip) -> operand for the next convolution
-      if (op.inorm[i] < 0 || c.cout % 8) {
-        set_error("layer %s: a non-final convolution must be followed by InstanceNormalization (Cout %% 8 == 0)",
-                  c.name.c_str());
-        return FAV_ERR_UNSUPPORTED;
-      }
-      PlanStep ns;
-      ns.kind = 1; ns.inorm = op.inorm[i]; ns.raw = raw; ns.stats_off = stats_off;
-      stats_off += 2 * c.cout;
-      const ConvDef *consumer = pos + 1 < order.size() ? &net->convs[order[pos + 1]] : nullptr;
-      FAV_TRY(make_operand(*pl, c.cout, ho, wo, consumer, &ns.dst));
-      if (op.kind == 1) {
-        ns.relu = i == 0 ? 1 : (op.relu ? 1 : 0);               // CX: needs_relu after the block (models_video.lua:108)
-        ns.skip = (i == 1 && op.skip) ? block_in : -1;          // RX: ShaveImage(2) / Identity of the block input (:46-50)
-        ns.shave = op.shave;
-      } else {
-        ns.relu = op.relu ? 1 : 0;
-      }
       cur = ns.dst;
       if (i == n - 1) { ns.layer_index = (int)oi; pl->layer_operand[(int)oi] = cur; }
       pl->steps.push_back(std::move(ns));
@@ -429,6 +509,19 @@ struct ProfRec {
   cudaEvent_t e0, e1;
 };
 
+// the raw tensors of a batch-normalized net, which only the CUDA-core comparator writes: allocated at its first run
+static int ensure_raw(Plan &pl) {
+  if (pl.raw_buf) return FAV_OK;
+  FAV_TRY(alloc_zero(pl, (void **)&pl.raw_buf, pl.raw_bytes));
+  FAV_TRY(alloc_zero(pl, (void **)&pl.raw_buf2, pl.raw_bytes));
+  for (PlanStep &s : pl.steps) {
+    float *p = s.raw_sel ? pl.raw_buf2 : pl.raw_buf;
+    s.raw.p = p;
+    for (SimtJob &j : s.simt) j.raw = p;
+  }
+  return FAV_OK;
+}
+
 // in7 == nullptr: the caller has already written the first operand (fused temporal input, run_plan_frame)
 static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int final_mode, cudaStream_t st,
                     std::vector<ProfRec> *prof = nullptr) {
@@ -447,7 +540,8 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
     if (!prof) return FAV_OK;
     return check_cuda(cudaEventRecord(prof->back().e1, st), "cudaEventRecord");
   };
-  FAV_TRY(check_cuda(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st), "cudaMemsetAsync(stats)"));
+  if (net->bn && net->conv_impl != 0) FAV_TRY(ensure_raw(pl));
+  if (!net->bn) FAV_TRY(check_cuda(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st), "cudaMemsetAsync(stats)"));
   if (in7) {
     FAV_TRY(begin(0, (double)pl.ops[0].H * pl.ops[0].W * (4.0 * net->in_dim + 32.0), "pack_input"));
     FAV_TRY(launch_pack_input(in7, net->in_dim, pl.H, pl.W, net->reflect_pad, pl.ops[0], st));
@@ -477,11 +571,20 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
       const InDef &n = net->inorms[s.inorm];
       const Operand &src = pl.ops[s.src];
       FAV_TRY(begin(3, 12.0 * n.C * src.H * src.W * (1.0 + s.scale * s.scale) / 2.0, n.name + ".up"));
-      FAV_TRY(launch_up_in(src, pl.stats + s.stats_off, n.d_gamma, n.d_beta, 1e-5f, s.relu, s.scale, pl.ops[s.dst], st));
+      FAV_TRY(launch_up_in(src, pl.stats + s.stats_off, n.d_gamma, n.d_beta, 1e-5f, s.relu, s.scale, pl.ops[s.dst], st, n.d_mean,
+                           n.d_scale));
       FAV_TRY(end());
     } else {
       if (s.fused_nl && net->conv_impl == 0) continue;  // the consumer conv normalises while it loads (norm-on-load)
       const InDef &n = net->inorms[s.inorm];
+      if (net->bn) {  // BatchNorm folded into the conv: its tensor-core epilogue wrote the operand
+        if (net->conv_impl == 0) continue;
+        FAV_TRY(begin(3, (s.skip >= 0 ? 12.0 : 8.0) * n.C * s.raw.H * s.raw.W, n.name + ".apply"));
+        FAV_TRY(launch_in_apply(s.raw, nullptr, nullptr, nullptr, 0.f, s.relu, s.skip >= 0 ? &pl.ops[s.skip] : nullptr, s.shave,
+                                pl.ops[s.dst], st));
+        FAV_TRY(end());
+        continue;
+      }
       double *sums = pl.stats + s.stats_off;
       const double elems = (double)n.C * s.raw.H * s.raw.W;
       if (net->conv_impl != 0) {  // the tcgen05 epilogue already accumulated the statistics
@@ -555,7 +658,16 @@ static int run_plan_frame(fav_net *net, Plan &pl, const float *src7, float *out3
 extern "C" {
 
 int fav_net_create(const char *arch, const char *padding_type, float tanh_constant, int in_dim, fav_net_t **out) {
+  return fav_net_create_norm(arch, padding_type, tanh_constant, in_dim, "instance", out);
+}
+
+int fav_net_create_norm(const char *arch, const char *padding_type, float tanh_constant, int in_dim, const char *norm,
+                        fav_net_t **out) {
   FAV_REQUIRE(arch && out, "fav_net_create: null argument");
+  // train_video.lua:22 -use_instance_norm: 1 = InstanceNormalization, 0 = SpatialBatchNormalization (models_video.lua:21-25,
+  // 33-37,121-127), which get_model runs in evaluate mode (fast_artistic_video_core.lua:46)
+  const std::string nt = norm ? norm : "instance";
+  FAV_REQUIRE(nt == "instance" || nt == "batch", "fav_net_create_norm: norm must be 'instance' or 'batch' (got '%s')", nt.c_str());
   FAV_REQUIRE(in_dim >= 1 && in_dim <= 8, "fav_net_create: in_dim must be in [1,8] (video nets use 7, image nets 3)");
   // models_video.lua:13-19,27-31,46-50,71-79: 'reflect-start' (every released video model; train_video.lua:25) = unpadded
   // residual convs + ShaveImage(2) + one lazily inserted reflection pad (train_video.lua:319-324); 'zero' = residual convs with
@@ -569,7 +681,7 @@ int fav_net_create(const char *arch, const char *padding_type, float tanh_consta
   }
   const bool zero_pad = ptype == "zero";
   std::unique_ptr<fav_net> net(new fav_net());
-  net->arch = arch; net->tanh_c = tanh_constant; net->in_dim = in_dim; net->padding_type = ptype;
+  net->arch = arch; net->tanh_c = tanh_constant; net->in_dim = in_dim; net->padding_type = ptype; net->bn = nt == "batch";
   // tokenise (models_video.lua:56)
   std::vector<std::string> toks;
   {
@@ -612,7 +724,7 @@ int fav_net_create(const char *arch, const char *padding_type, float tanh_consta
       FAV_REQUIRE(sc >= 1 && sc <= 4 && !op.last && prev % 8 == 0, "bad arch token '%s'", v.c_str());
       next = prev;
       op.kind = 2; op.scale = sc;
-      op.inorm[0] = add_in(net.get(), name + ".n", next);
+      op.inorm[0] = add_in(net.get(), name + ".n", next, -1);
       needs_bn = false;
       scale /= sc;
     } else if (c0 == 'f' && v.size() >= 6 && v[2] == 's' && v[4] == '-') {  // fXsY-Z  :81-89  SpatialFullConvolution(f,f,s,s,p,p,s-1,s-1)
@@ -629,9 +741,9 @@ int fav_net_create(const char *arch, const char *padding_type, float tanh_consta
       op.skip = c0 == 'R';
       op.shave = zero_pad ? 0 : 2;      // ShaveImage(2) vs Identity :46-50
       op.conv[0] = add_conv(net.get(), name + ".c1", prev, next, 3, 1, bp, false, 0);
-      op.inorm[0] = add_in(net.get(), name + ".n1", next);
+      op.inorm[0] = add_in(net.get(), name + ".n1", next, op.conv[0]);
       op.conv[1] = add_conv(net.get(), name + ".c2", next, next, 3, 1, bp, false, 0);
-      op.inorm[1] = add_in(net.get(), name + ".n2", next);
+      op.inorm[1] = add_in(net.get(), name + ".n2", next, op.conv[1]);
       needs_bn = false; op.relu = c0 == 'C';  // :107-108, :113-114
       if (!zero_pad) shrink += 4 * scale;
     } else {
@@ -639,7 +751,7 @@ int fav_net_create(const char *arch, const char *padding_type, float tanh_consta
       return FAV_ERR_UNSUPPORTED;
     }
     if (op.last) { needs_bn = false; op.relu = false; }  // :117-120
-    if (needs_bn && op.kind == 0) op.inorm[0] = add_in(net.get(), name + ".n", next);
+    if (needs_bn && op.kind == 0) op.inorm[0] = add_in(net.get(), name + ".n", next, op.conv[0]);
     net->ops.push_back(op);
     prev = next;
   }
@@ -689,6 +801,8 @@ int fav_net_finalize(fav_net_t *net) {
   FAV_REQUIRE(net, "fav_net_finalize: null net");
   if (net->finalized) return FAV_OK;
   for (Param &p : net->params) FAV_REQUIRE(p.set, "fav_net_finalize: parameter %s was never set", p.name.c_str());
+  std::vector<std::vector<float>> cw, cb, cs;
+  FAV_TRY(fold_batch_norms(net, cw, cb, cs));
   // K-step tables (N blocks for Cout > 128) of every convolution, before any device work: a layer the tensor-core path
   // cannot run is refused here, by name, rather than at the first forward
   for (ConvDef &c : net->convs) FAV_TRY(plan_conv_nblocks(c));
@@ -701,10 +815,15 @@ int fav_net_finalize(fav_net_t *net) {
     return FAV_ERR_UNSUPPORTED;
   }
   net->num_sms = prop.multiProcessorCount;
-  for (ConvDef &c : net->convs) FAV_TRY(pack_conv_weights(net, c));
+  for (size_t i = 0; i < net->convs.size(); ++i)
+    FAV_TRY(pack_conv_weights(net, net->convs[i], net->params[net->convs[i].pw].host, cb[i], cw[i], cs[i]));
   for (InDef &n : net->inorms) {
     FAV_TRY(dev_upload(net, net->params[n.pw].host, &n.d_gamma));
     FAV_TRY(dev_upload(net, net->params[n.pb].host, &n.d_beta));
+    if (!n.h_scale.empty()) {
+      FAV_TRY(dev_upload(net, n.h_mean, &n.d_mean));
+      FAV_TRY(dev_upload(net, n.h_scale, &n.d_scale));
+    }
   }
   net->finalized = true;
   return FAV_OK;

@@ -136,11 +136,15 @@ __global__ void __launch_bounds__(128) in_apply_kernel(RawTensor raw, const doub
       }
     }
   }
-  // 2. mean / gamma * rstd / beta of the block's 8 channels
+  // 2. mean / gamma * rstd / beta of the block's 8 channels (no sums: identity, the BatchNorm is folded into the conv)
   if (threadIdx.x < 8) {
     int c = cb * 8 + threadIdx.x;
-    in_finalize(sums[c], sums[raw.C + c], inv_count, eps, gamma[c], s_mean[threadIdx.x], s_scale[threadIdx.x]);
-    s_beta[threadIdx.x] = beta[c];
+    if (sums) {
+      in_finalize(sums[c], sums[raw.C + c], inv_count, eps, gamma[c], s_mean[threadIdx.x], s_scale[threadIdx.x]);
+      s_beta[threadIdx.x] = beta[c];
+    } else {
+      s_mean[threadIdx.x] = 0.f; s_scale[threadIdx.x] = 1.f; s_beta[threadIdx.x] = 0.f;
+    }
   }
   __syncthreads();
   // 3. normalise (+ReLU) (+skip), split into fp16 hi / lo, store the next operand
@@ -231,13 +235,18 @@ __global__ void __launch_bounds__(256) opnd_stats_kernel(Operand src, double *__
 
 __global__ void __launch_bounds__(128) up_apply_kernel(Operand src, const double *__restrict__ sums,
                                                        const float *__restrict__ gamma, const float *__restrict__ beta,
-                                                       double inv_count, double eps, int relu, int scale, Operand dst) {
+                                                       double inv_count, double eps, int relu, int scale, Operand dst,
+                                                       const float *__restrict__ tab_mean, const float *__restrict__ tab_scale) {
   __shared__ float s_mean[8], s_scale[8], s_beta[8];
   const int xbase = blockIdx.x * (128 * kApplyIter) + threadIdx.x;
   const int y = blockIdx.y, cb = blockIdx.z;
   if (threadIdx.x < 8) {
     int c = cb * 8 + threadIdx.x;
-    in_finalize(sums[c], sums[src.C + c], inv_count, eps, gamma[c], s_mean[threadIdx.x], s_scale[threadIdx.x]);
+    if (tab_scale) {  // inference-mode BatchNorm after the upsampling: running mean, weight / sqrt(running_var + eps)
+      s_mean[threadIdx.x] = tab_mean[c]; s_scale[threadIdx.x] = tab_scale[c];
+    } else {
+      in_finalize(sums[c], sums[src.C + c], inv_count, eps, gamma[c], s_mean[threadIdx.x], s_scale[threadIdx.x]);
+    }
     s_beta[threadIdx.x] = beta[c];
   }
   __syncthreads();
@@ -259,11 +268,14 @@ __global__ void __launch_bounds__(128) up_apply_kernel(Operand src, const double
 }
 
 int launch_up_in(const Operand &src, double *sums, const float *gamma, const float *beta, float eps, int relu, int scale,
-                 const Operand &dst, cudaStream_t st) {
-  opnd_stats_kernel<<<dim3(src.Cb, ceil_div(src.H, kStatRows)), 256, 0, st>>>(src, sums);
-  FAV_TRY(post_launch("up_in.stats"));
+                 const Operand &dst, cudaStream_t st, const float *tab_mean, const float *tab_scale) {
+  if (!tab_scale) {
+    opnd_stats_kernel<<<dim3(src.Cb, ceil_div(src.H, kStatRows)), 256, 0, st>>>(src, sums);
+    FAV_TRY(post_launch("up_in.stats"));
+  }
   dim3 grid(ceil_div(dst.W, 128 * kApplyIter), dst.H, dst.Cb);
-  up_apply_kernel<<<grid, 128, 0, st>>>(src, sums, gamma, beta, 1.0 / ((double)src.H * src.W), (double)eps, relu, scale, dst);
+  up_apply_kernel<<<grid, 128, 0, st>>>(src, sums, gamma, beta, 1.0 / ((double)src.H * src.W), (double)eps, relu, scale, dst,
+                                        tab_mean, tab_scale);
   return post_launch("up_in.apply");
 }
 

@@ -15,6 +15,8 @@
 //  Raw      fp32 convolution output before InstanceNorm: [Ho][Cq][Wp][4 channels] -- 16 bytes per
 //           (pixel, channel-quad); the epilogue writes the two channels a thread holds as one 8-byte store.
 //           RawTensor::planar (fp32 [C][Hp][Wp]) is a layout the normalisation kernels also accept.
+//           Batch-normalized nets have no raw tensors on the tensor-core path: the BN is folded into the conv and the conv
+//           epilogue writes the next operand itself (ConvJob::opnd).
 #pragma once
 #include "fav_common.cuh"
 #include <cuda_fp16.h>
@@ -35,6 +37,9 @@ struct Operand {
     int64_t base = ((int64_t)ys * Cb + cb) * slab16();
     return base + (parity ? (int64_t)(xs & 1) * Ws2 + (xs >> 1) : xs);
   }
+  // offset in 4-byte units (one fp16 pair of hi or of lo) of channels (c, c + 1), c even, of logical pixel (y, x): where the
+  // operand epilogue of conv_tc_kernel stores, and reads the skip from.  Interior pixels only, so the zero border stays.
+  __host__ __device__ int64_t pair_off4(int y, int x, int c) const { return off16(padT + y, c >> 3, padL + x) * 4 + ((c & 7) >> 1); }
 };
 
 #ifdef __CUDACC__

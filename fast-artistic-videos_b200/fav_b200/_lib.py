@@ -74,6 +74,7 @@ SIGNATURES = {
     "fav_pnm_read_u8": (C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "fav_flo_read_raw": (C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "fav_net_create": (C.c_int, [C.c_char_p, C.c_char_p, C.c_float, C.c_int, C.POINTER(C.c_void_p)]),
+    "fav_net_create_norm": (C.c_int, [C.c_char_p, C.c_char_p, C.c_float, C.c_int, C.c_char_p, C.POINTER(C.c_void_p)]),
     "fav_net_destroy": (None, [C.c_void_p]),
     "fav_net_num_params": (C.c_int, [C.c_void_p]),
     "fav_net_param_info": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, _i64p, _i64p]),

@@ -44,7 +44,8 @@ def load_model(path_or_style: str, arch: str = synth.DEFAULT_ARCH, in_dim: int =
         import numpy as np
 
         w = dict(np.load(path_or_style))
-        return models_video.StyleNet(arch, in_dim=in_dim).load_state(w)
+        norm = "batch" if any(k.endswith(".running_var") for k in w) else "instance"
+        return models_video.StyleNet(arch, in_dim=in_dim, norm=norm).load_state(w)
     if path_or_style.endswith(".t7"):  # torch.load(path).model (core.lua:39-47)
         from . import t7
 
@@ -54,7 +55,7 @@ def load_model(path_or_style: str, arch: str = synth.DEFAULT_ARCH, in_dim: int =
         except t7.GeometryError as e:  # a padding_type / module layout this implementation does not run
             raise _lib.FavError(_lib.FAV_ERR_UNSUPPORTED, str(e)) from None
         cin = int(next(v for k, v in state.items() if k == "l0.weight").shape[1])
-        net = models_video.StyleNet(t7_arch, geo["padding_type"], tanh_constant=tanh_c, in_dim=cin)
+        net = models_video.StyleNet(t7_arch, geo["padding_type"], tanh_constant=tanh_c, in_dim=cin, norm=geo["norm"])
         want = synth.reflect_start_pad(synth.parse_arch(t7_arch, cin), geo["padding_type"])
         if pad != want:  # the file's SpatialReflectionPadding must be the one the arch implies (train_video.lua:319-324)
             raise _lib.FavError(_lib.FAV_ERR_UNSUPPORTED, f"{path_or_style}: SpatialReflectionPadding({pad}) in the checkpoint, "

@@ -16,13 +16,16 @@ from . import _lib, synth
 
 class StyleNet:
     def __init__(self, arch: str = synth.DEFAULT_ARCH, padding_type: str = "reflect-start",
-                 tanh_constant: float = 150.0, in_dim: int = 7):
+                 tanh_constant: float = 150.0, in_dim: int = 7, norm: str = "instance"):
+        """norm: 'instance' (InstanceNormalization, the default) or 'batch' (SpatialBatchNormalization in evaluate mode,
+        -use_instance_norm 0; its parameters add '<n>.running_mean', '<n>.running_var' and '<n>.eps')."""
         h = C.c_void_p()
-        _lib.check(_lib.lib.fav_net_create(arch.encode(), padding_type.encode(), C.c_float(tanh_constant), in_dim,
-                                           C.byref(h)))
+        _lib.check(_lib.lib.fav_net_create_norm(arch.encode(), padding_type.encode(), C.c_float(tanh_constant), in_dim,
+                                                norm.encode(), C.byref(h)))
         self._h = h
         self.arch = arch
         self.in_dim = in_dim
+        self.norm = norm
         self.finalized = False
 
     def __del__(self):
@@ -133,13 +136,11 @@ class StyleNet:
 def build_model(opt) -> StyleNet:
     """M.build_model(opt) (models_video.lua:55): opt.arch, opt.padding_type, opt.tanh_constant, opt.use_instance_norm."""
     get = (lambda k, d: opt.get(k, d)) if isinstance(opt, dict) else (lambda k, d: getattr(opt, k, d))
-    if int(get("use_instance_norm", 1)) != 1:
-        raise _lib.FavError(_lib.FAV_ERR_UNSUPPORTED, "use_instance_norm=0 (batch norm) is not on the inference path")
     return StyleNet(get("arch", synth.DEFAULT_ARCH), get("padding_type", "reflect-start"),
-                    float(get("tanh_constant", 150.0)))
+                    float(get("tanh_constant", 150.0)), norm="instance" if int(get("use_instance_norm", 1)) == 1 else "batch")
 
 
-def synthetic_model(style: str = "candy", arch: str = synth.DEFAULT_ARCH, in_dim: int = 7) -> StyleNet:
+def synthetic_model(style: str = "candy", arch: str = synth.DEFAULT_ARCH, in_dim: int = 7, norm: str = "instance") -> StyleNet:
     """Seeded random-init weights for a named style (no network => no released checkpoints; SURVEY.md §8c).
     in_dim = 3: an image model (-model_img) of the same architecture."""
-    return StyleNet(arch, in_dim=in_dim).load_state(synth.make_weights(arch, style, in_dim))
+    return StyleNet(arch, in_dim=in_dim, norm=norm).load_state(synth.make_weights(arch, style, in_dim, norm))

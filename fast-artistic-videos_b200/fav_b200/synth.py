@@ -8,6 +8,7 @@ Weights follow Torch7's own module initialisers, which is what a freshly built
 `models_video.build_model` (fast_artistic_video/models_video.lua:55-140) holds:
   nn.SpatialConvolution / SpatialFullConvolution reset(): U(-s, s), s = 1/sqrt(kW*kH*nInputPlane)
   nn.InstanceNormalization: weight ~ U[0,1), bias = 0   (InstanceNormalization.lua:26-27)
+  nn.SpatialBatchNormalization (norm='batch'): the same, plus running_mean = 0, running_var = 1, eps = 1e-5
 One seed per style name ("candy", "mosaic", "scream", ...).
 """
 from __future__ import annotations
@@ -91,8 +92,10 @@ def reflect_start_pad(specs, padding_type: str = "reflect-start") -> int:
     return int(shrink) // 2
 
 
-def make_weights(arch: str = DEFAULT_ARCH, style: str = "candy", in_dim: int = 7):
-    """Dict name -> fp32 array.  conv: (cout,cin,k,k); fullconv: (cin,cout,k,k) (Torch layout)."""
+def make_weights(arch: str = DEFAULT_ARCH, style: str = "candy", in_dim: int = 7, norm: str = "instance"):
+    """Dict name -> fp32 array.  conv: (cout,cin,k,k); fullconv: (cin,cout,k,k) (Torch layout).  norm='batch' adds each norm's
+    running statistics and eps; every other array (and the random stream) is the one norm='instance' gives."""
+    assert norm in ("instance", "batch")
     rng = np.random.default_rng(style_seed(style))
     specs = parse_arch(arch, in_dim)
     w = {}
@@ -106,6 +109,10 @@ def make_weights(arch: str = DEFAULT_ARCH, style: str = "candy", in_dim: int = 7
     def in_w(name, c):
         w[name + ".weight"] = rng.uniform(0.0, 1.0, size=(c,)).astype(np.float32)
         w[name + ".bias"] = np.zeros((c,), np.float32)
+        if norm == "batch":
+            w[name + ".running_mean"] = np.zeros((c,), np.float32)
+            w[name + ".running_var"] = np.ones((c,), np.float32)
+            w[name + ".eps"] = np.full((1,), 1e-5, np.float32)
 
     for i, s in enumerate(specs):
         n = f"l{i}"

@@ -132,6 +132,9 @@ def _mods(m) -> List:
     return [mods[k] for k in sorted(mods)]
 
 
+NORMS = ("InstanceNormalization", "SpatialBatchNormalization")  # nn.* / cudnn.* classes alike (_cls drops the package)
+
+
 class GeometryError(ValueError):
     """The checkpoint's module tree does not have the geometry build_model would give its arch string."""
 
@@ -143,10 +146,14 @@ def model_to_state(model, geometry: dict = None) -> Tuple[str, Dict[str, np.ndar
     padding: 'padding_type' ('reflect-start' | 'zero', inferred from the residual blocks: pad-0 convs + ShaveImage vs pad-1
     convs + Identity, models_video.lua:21-53), 'has_reflect_pad', and every conv's (name, padW, padW implied by its token);
     a layout build_model cannot produce for these two padding types raises GeometryError instead of being run with a
-    different geometry."""
+    different geometry.  geometry['norm'] is 'instance' (InstanceNormalization) or 'batch' (nn. / cudnn.SpatialBatchNormalization,
+    -use_instance_norm 0, models_video.lua:21-25,33-37,121-127: weight / bias, nil when affine = false, are read as 1 / 0, plus
+    running_mean, running_var and eps); a checkpoint mixing the two, a BatchNorm without running statistics or one whose size
+    is not its convolution's output channel count raises GeometryError."""
     toks, state, tanh_c, pad = [], {}, 150.0, 0
     geo = geometry if geometry is not None else {}
-    geo.update(padding_type=None, has_reflect_pad=False, conv_pads=[])
+    geo.update(padding_type=None, has_reflect_pad=False, conv_pads=[], norm=None)
+    chan = None  # output channels of the last convolution
 
     def check_pad(name, m, implied):
         pw, ph = int(m.get("padW", 0)), int(m.get("padH", m.get("padW", 0)))
@@ -157,18 +164,41 @@ def model_to_state(model, geometry: dict = None) -> Tuple[str, Dict[str, np.ndar
     i = 0
 
     def conv_params(name, m, transposed):
+        nonlocal chan
         w = np.asarray(m["weight"], np.float32)
         cin, cout, k = int(m["nInputPlane"]), int(m["nOutputPlane"]), int(m["kW"])
+        chan = cout
         state[name + ".weight"] = w.reshape((cin, cout, k, k) if transposed else (cout, cin, k, k))
         state[name + ".bias"] = np.asarray(m["bias"], np.float32).reshape(cout)
 
     def in_params(name, m):
-        state[name + ".weight"] = np.asarray(m["weight"], np.float32).reshape(-1)
-        state[name + ".bias"] = np.asarray(m["bias"], np.float32).reshape(-1)
+        kind = "batch" if _cls(m) == "SpatialBatchNormalization" else "instance"
+        if geo["norm"] not in (None, kind):
+            raise GeometryError(f".t7 model: {name} is a {m.torch_type} after {geo['norm']} normalisation layers; a checkpoint "
+                                "uses one normalisation type throughout (-use_instance_norm, train_video.lua:22)")
+        geo["norm"] = kind
+        if kind == "instance":
+            state[name + ".weight"] = np.asarray(m["weight"], np.float32).reshape(-1)
+            state[name + ".bias"] = np.asarray(m["bias"], np.float32).reshape(-1)
+            return
+        for f in ("running_mean", "running_var"):  # evaluate mode normalises with the running statistics
+            if m.get(f) is None:
+                raise GeometryError(f".t7 model: {name} ({m.torch_type}) has no {f}")
+        mean = np.asarray(m["running_mean"], np.float32).reshape(-1)
+        var = np.asarray(m["running_var"], np.float32).reshape(-1)
+        if not mean.size == var.size == chan:
+            raise GeometryError(f".t7 model: {name} ({m.torch_type}) has {var.size} channels, its convolution {chan}")
+        w, b = m.get("weight"), m.get("bias")  # nil when affine = false
+        state[name + ".weight"] = np.ones(chan, np.float32) if w is None else np.asarray(w, np.float32).reshape(-1)
+        state[name + ".bias"] = np.zeros(chan, np.float32) if b is None else np.asarray(b, np.float32).reshape(-1)
+        if not state[name + ".weight"].size == state[name + ".bias"].size == chan:
+            raise GeometryError(f".t7 model: {name} ({m.torch_type}) weight / bias do not have {chan} channels")
+        state[name + ".running_mean"], state[name + ".running_var"] = mean, var
+        state[name + ".eps"] = np.full(1, m.get("eps", 1e-5), np.float32)
 
     def take_norm_relu(name):
         nonlocal i
-        if i < len(mods) and _cls(mods[i]) == "InstanceNormalization":
+        if i < len(mods) and _cls(mods[i]) in NORMS:
             in_params(name + ".n", mods[i])
             i += 1
         if i < len(mods) and _cls(mods[i]) == "ReLU":
@@ -207,9 +237,9 @@ def model_to_state(model, geometry: dict = None) -> Tuple[str, Dict[str, np.ndar
             concat = _mods(m)[0]
             block = _mods(_mods(concat)[0])
             convs = [b for b in block if _cls(b) == "SpatialConvolution"]
-            norms = [b for b in block if _cls(b) == "InstanceNormalization"]
+            norms = [b for b in block if _cls(b) in NORMS]
             assert len(convs) == 2 and len(norms) == 2, "unexpected residual block layout"
-            extra = [_cls(b) for b in block if _cls(b) not in ("SpatialConvolution", "InstanceNormalization", "ReLU")]
+            extra = [_cls(b) for b in block if _cls(b) not in ("SpatialConvolution", "ReLU") + NORMS]
             skip = _cls(_mods(concat)[1]) if len(_mods(concat)) > 1 else None
             rp = int(convs[0].get("padW", 0))
             ptype = "reflect-start" if (rp == 0 and skip == "ShaveImage") else ("zero" if (rp == 1 and skip == "Identity") else None)
@@ -230,6 +260,8 @@ def model_to_state(model, geometry: dict = None) -> Tuple[str, Dict[str, np.ndar
             pass  # identity in forward (TotalVariation.lua:12-15)
         else:
             raise ValueError(f".t7 model: unsupported module {m.torch_type}")
+    if geo["norm"] is None:
+        geo["norm"] = "instance"
     if geo["padding_type"] is None:
         geo["padding_type"] = "reflect-start" if geo["has_reflect_pad"] else "zero"
     if geo["has_reflect_pad"] != (geo["padding_type"] == "reflect-start" and pad > 0) and any(t[0] in "RC" for t in toks):
@@ -292,10 +324,12 @@ class _Writer:
 
 
 def write_checkpoint(path: str, arch: str, state: Dict[str, np.ndarray], tanh_constant: float = 150.0,
-                     reflect_pad: int = 40, padding_type: str = "reflect-start") -> None:
+                     reflect_pad: int = 40, padding_type: str = "reflect-start", norm: str = "instance",
+                     bn_class: str = "nn.SpatialBatchNormalization", affine: bool = True) -> None:
     """Serialise a state dict as the `{model = nn.Sequential{...}}` table train_video.lua:507-541 saves
     (padding_type 'reflect-start': leading reflection pad, pad-0 residual convs + ShaveImage; 'zero': pad-1 residual convs +
-    Identity, models_video.lua:21-53)."""
+    Identity, models_video.lua:21-53).  norm='batch': `bn_class` modules (nn. or cudnn.SpatialBatchNormalization) with the
+    state's running_mean / running_var / eps, in evaluate mode; affine=False leaves weight and bias nil."""
     from . import synth
 
     def seq(mods, cls="nn.Sequential"):
@@ -307,6 +341,12 @@ def write_checkpoint(path: str, arch: str, state: Dict[str, np.ndarray], tanh_co
                          "weight": state[name + ".weight"], "bias": state[name + ".bias"]})
 
     def inorm(name):
+        if norm == "batch":
+            f = {"running_mean": state[name + ".running_mean"], "running_var": state[name + ".running_var"],
+                 "eps": float(state[name + ".eps"].reshape(-1)[0]), "momentum": 0.1, "affine": affine, "train": False}
+            if affine:
+                f.update(weight=state[name + ".weight"], bias=state[name + ".bias"])
+            return T7Object(bn_class, f)
         return T7Object("nn.InstanceNormalization", {"weight": state[name + ".weight"], "bias": state[name + ".bias"],
                                                       "eps": 1e-5, "nOutput": int(state[name + ".weight"].size)})
 
@@ -334,7 +374,10 @@ def write_checkpoint(path: str, arch: str, state: Dict[str, np.ndarray], tanh_co
     mods += [T7Object("nn.Tanh", {}), T7Object("nn.MulConstant", {"constant_scalar": tanh_constant}),
              T7Object("nn.TotalVariation", {"strength": 1e-6})]
     w = _Writer()
-    w.obj({"opt": {"arch": arch, "padding_type": padding_type}, "iter": 60000, "model": seq(mods)})
+    opt = {"arch": arch, "padding_type": padding_type}
+    if norm == "batch":
+        opt["use_instance_norm"] = 0
+    w.obj({"opt": opt, "iter": 60000, "model": seq(mods)})
     with open(path, "wb") as f:
         f.write(bytes(w.b))
 

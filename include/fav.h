@@ -181,6 +181,14 @@ typedef struct fav_net fav_net_t;
 
 FAV_API int fav_net_create(const char *arch, const char *padding_type, float tanh_constant, int in_dim,
                            fav_net_t **out);
+/* fav_net_create with the normalisation layer chosen by -use_instance_norm (train_video.lua:22): norm "instance"
+ * (= fav_net_create) or "batch", nn.SpatialBatchNormalization wherever the default has InstanceNormalization
+ * (models_video.lua:21-25,33-37,121-127), run in evaluate mode (fast_artistic_video_core.lua:46): y = (x - running_mean) /
+ * sqrt(running_var + eps) * weight + bias.  Each norm "<n>" then has the parameters "<n>.weight|bias|running_mean|running_var"
+ * [C] and "<n>.eps" [1].  fav_net_finalize folds every BN that follows a convolution into that convolution (its bias and a
+ * per-channel scale) and refuses (FAV_ERR_INVALID, naming the norm) non-finite values or running_var + eps <= 0. */
+FAV_API int fav_net_create_norm(const char *arch, const char *padding_type, float tanh_constant, int in_dim, const char *norm,
+                                fav_net_t **out);
 FAV_API void fav_net_destroy(fav_net_t *net);
 FAV_API int fav_net_num_params(const fav_net_t *net);
 /* name_out: >= 64 bytes; shape_out[4] (unused dims = 1); returns element count via *numel */
