@@ -101,22 +101,50 @@ struct ConvJob {
   // channel epi_c0 + c of epi_dst, the next convolution's operand.  epi_c0: the N block's first channel.
   int opnd, epi_relu, epi_skip, epi_shave, epi_c0;
   const float *epi_scale;
-  Operand epi_dst, epi_skip_op;
+  Operand epi_dst, epi_skip_op;  // per-image strides: Operand::img16
+  // a batch of nimg images of one size (tile_at): image b of every tensor starts b * <stride> elements in -- the A operand
+  // (16-byte units), raw (floats), out3 (floats), stats (doubles), nl_raw (float4 units), nl_sums (doubles)
+  int nimg;
+  int64_t a_img16, raw_img, out3_img, stats_img, nl_raw_img4, nl_sums_img;
 };
 
-// Operand epilogue addressing, shared by conv_tc_kernel and its CPU emulator (tests/emu/opnd_epi_emu.cu).  Consumer thread t
-// (0..255) of a tile holds, for i < Npad / 8 and h < 2, the accumulator pair of channels c, c + 1 (c = 8i + 2 (t % 4)) of tile
+// Tile T of a batched job, T = b * ntiles + t for image b and tile t of that image's output (0 <= T < nimg * ntiles): every role
+// of conv_tc_kernel (consumers, patch / weight / norm-on-load producers) walks T = blockIdx.x, blockIdx.x + gridDim.x, ... and
+// decodes it here, as does the CPU emulator (tests/emu/batch_emu.cu).  y / x0: the tile's output row and first output column;
+// the rest: image b's base offsets into each tensor of the job.
+struct TileAt {
+  int b, y, x0;
+  int64_t a16, raw, out3, stats, nl_raw4, nl_sums;  // the operand epilogue's: opnd_epi_addr
+};
+// batch == false: a single-image launch (nimg == 1, T = t), decoded without the division by ntiles
+__host__ __device__ inline TileAt tile_at(const ConvJob &j, int T, bool batch = true) {
+  TileAt a;
+  a.b = batch ? T / j.ntiles : 0;
+  const int t = T - a.b * j.ntiles;
+  a.y = t / j.tiles_x;
+  a.x0 = (t - a.y * j.tiles_x) * j.tile_dx;
+  a.a16 = a.b * j.a_img16; a.raw = a.b * j.raw_img; a.out3 = a.b * j.out3_img; a.stats = a.b * j.stats_img;
+  a.nl_raw4 = a.b * j.nl_raw_img4; a.nl_sums = a.b * j.nl_sums_img;
+  return a;
+}
+
+// Operand epilogue addressing, shared by conv_tc_kernel and its CPU emulators (tests/emu/opnd_epi_emu.cu, batch_emu.cu).  tile:
+// the batched tile index T of tile_at.  Consumer thread t (0..255) of a tile holds, for i < Npad / 8 and h < 2, the accumulator pair of channels c, c + 1 (c = 8i + 2 (t % 4)) of tile
 // pixel r0 + 8h (r0 = 64 (t / 128) + 16 (t / 32 % 4) + t % 32 / 4).  Returns false when that pair lies outside the job's
 // output (no store); else the 4-byte offsets of its fp16 pair in the hi / lo planes of epi_dst and, for a residual skip, of
 // epi_skip_op.
-__host__ __device__ inline bool opnd_epi_addr(const ConvJob &j, int tile, int t, int i, int h, int64_t &dst4, int64_t &skip4) {
-  const int y = tile / j.tiles_x, x = (tile - y * j.tiles_x) * j.tile_dx + (t >> 7) * 64 + ((t >> 5) & 3) * 16 + ((t & 31) >> 2) + 8 * h;
+__host__ __device__ inline bool opnd_epi_addr(const ConvJob &j, const TileAt &at, int t, int i, int h, int64_t &dst4, int64_t &skip4) {
+  const int y = at.y, x = at.x0 + (t >> 7) * 64 + ((t >> 5) & 3) * 16 + ((t & 31) >> 2) + 8 * h;
   const int c = 8 * i + 2 * (t & 3);
   if (x >= j.Wo || y >= j.Ho || c >= j.Cout) return false;
   const int yo = y * j.oy_mul + j.oy_off, xo = x * j.ox_mul + j.ox_off;
-  dst4 = j.epi_dst.pair_off4(yo, xo, j.epi_c0 + c);
-  skip4 = j.epi_skip ? j.epi_skip_op.pair_off4(yo + j.epi_shave, xo + j.epi_shave, j.epi_c0 + c) : 0;
+  dst4 = at.b * j.epi_dst.img16 * 4 + j.epi_dst.pair_off4(yo, xo, j.epi_c0 + c);
+  skip4 = j.epi_skip ? at.b * j.epi_skip_op.img16 * 4 + j.epi_skip_op.pair_off4(yo + j.epi_shave, xo + j.epi_shave, j.epi_c0 + c) : 0;
   return true;
+}
+__host__ __device__ inline bool opnd_epi_addr(const ConvJob &j, int tile, int t, int i, int h, int64_t &dst4, int64_t &skip4,
+                                              bool batch = true) {
+  return opnd_epi_addr(j, tile_at(j, tile, batch), t, i, h, dst4, skip4);
 }
 
 // CUDA-core comparator job (debug / bring-up path; same inputs and outputs as ConvJob)
@@ -147,14 +175,17 @@ size_t conv_tc_trace_used();
 void conv_tc_choose_slots(ConvJob &job);  // fills b_slots / b_resident from the shared-memory budget
 
 // elementwise / reduction kernels of the net (net_kernels.cu)
-int launch_pack_input(const float *in, int Cin, int H, int W, int reflect, const Operand &dst, cudaStream_t st);
-int launch_in_stats(const RawTensor &raw, double *sums /*[2*C]*/, cudaStream_t st);
+// nimg > 1: a batch of images of one size -- in [nimg][Cin][H][W]; raw, operands and sums per image (RawTensor::img,
+// Operand::img16, sums_img doubles apart)
+int launch_pack_input(const float *in, int Cin, int H, int W, int reflect, const Operand &dst, cudaStream_t st, int nimg = 1);
+int launch_in_stats(const RawTensor &raw, double *sums /*[2*C]*/, cudaStream_t st, int nimg = 1, int64_t sums_img = 0);
 // sums == null: no normalisation (batch-normalized nets on the CUDA-core comparator: ReLU / skip / pack only)
 int launch_in_apply(const RawTensor &raw, const double *sums, const float *gamma, const float *beta, float eps, int relu,
-                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st);
+                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st, int nimg = 1, int64_t sums_img = 0);
 // tab_mean / tab_scale non-null: a fixed per-channel affine (inference-mode BatchNorm) instead of the statistics of src
 int launch_up_in(const Operand &src, double *sums, const float *gamma, const float *beta, float eps, int relu, int scale,
-                 const Operand &dst, cudaStream_t st, const float *tab_mean = nullptr, const float *tab_scale = nullptr);
+                 const Operand &dst, cudaStream_t st, const float *tab_mean = nullptr, const float *tab_scale = nullptr,
+                 int nimg = 1, int64_t sums_img = 0);
 int launch_unpack_operand(const Operand &src, float *out_nchw, cudaStream_t st);
 
 }  // namespace fav

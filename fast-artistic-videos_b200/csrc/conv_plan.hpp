@@ -392,6 +392,11 @@ static inline void set_opnd_epilogue(ConvJob &j, int b, const float *scale, cons
   j.epi_skip = skip ? 1 : 0; j.epi_skip_op = skip ? *skip : Operand(); j.epi_shave = skip ? shave : 0;
   j.raw = nullptr; j.stats = nullptr;
 }
+// a batch of nimg images of one size (conv.cuh tile_at): per-image strides of the job's raw output (floats), final frame (floats)
+// and fused statistics (doubles); the A operand's and the operand epilogue's come with their Operands (Operand::img16)
+static inline void set_conv_batch(ConvJob &j, int nimg, int64_t raw_img, int64_t out3_img, int64_t stats_img) {
+  j.nimg = nimg; j.raw_img = raw_img; j.out3_img = out3_img; j.stats_img = stats_img;
+}
 // K-step tables of every phase of a stylization-net convolution, or of every N block's phases when Cout > kMaxNBlock.  A
 // geometry the tensor-core planner cannot run fails here with FAV_ERR_UNSUPPORTED and the layer's name.
 static inline int plan_conv_nblocks(ConvDef &c) {
@@ -495,6 +500,7 @@ static inline int fill_conv_job(const ConvDef &c, const ConvPhase &ph, const Ope
   conv_out_size(c, in.H, in.W, &Ho, &Wo);
   const int pHo = c.transposed ? in.H : Ho, pWo = c.transposed ? in.W : Wo;  // phase grid
   memset(&j, 0, sizeof(j));
+  j.nimg = 1; j.a_img16 = in.img16;
   j.a_hi = reinterpret_cast<const uint4 *>(in.hi); j.a_lo = reinterpret_cast<const uint4 *>(in.lo);
   j.a_Cb = in.Cb; j.a_slab16 = in.slab16();
   j.tile_dx = ph.kind == 3 ? kTileM - (c.k - 1) : kTileM;

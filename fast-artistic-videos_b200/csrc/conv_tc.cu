@@ -64,10 +64,33 @@ __device__ __forceinline__ void trace_put(const ConvJob &job, int word, long lon
   if (job.trace) job.trace[(size_t)blockIdx.x * kTraceWords + word] = (unsigned long long)v;
 }
 
+// fused statistics of image b: the 8 warps' partial sums added in a FIXED order (deterministic per CTA: the tile -> CTA assignment
+// is static), then one double atomic per channel and quantity per CTA.  reset: the partials are zeroed for the next image (thread
+// ch clears the column it has just read; the closing barrier keeps the next tile's writers behind it).
+__device__ __forceinline__ void tc_flush_stats(const ConvJob &job, float *slot, int b, bool reset) {
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  const int ch = threadIdx.x;
+  if (ch < job.Cout) {
+    float ssum = 0.f, qsum = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) { ssum += slot[w * 256 + ch]; qsum += slot[w * 256 + 128 + ch]; }
+    double *st = job.stats + b * job.stats_img;
+    atomicAdd(st + ch, (double)ssum);
+    atomicAdd(st + job.stats_pitch + ch, (double)qsum);
+  }
+  if (reset) {
+    if (ch < 128)
+#pragma unroll
+      for (int w = 0; w < 8; ++w) { slot[w * 256 + ch] = 0.f; slot[w * 256 + 128 + ch] = 0.f; }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+  }
+}
+
 // consumer warpgroup: MMAs of one 64-pixel half of every tile of this CTA, then its epilogue.
 // OPND: operand epilogue of batch-normalized nets (ConvJob::opnd) -- a template parameter, so the raw-output instances keep
-// their code and registers.
-template <int NT, bool OPND>
+// their code and registers.  BATCH: nimg > 1.  The same code; BATCH == false compiles it with nimg == 1 (one image, every
+// image offset zero), so a single-frame launch keeps the code of a kernel without batches (about 1.5 % of a 720p frame).
+template <int NT, bool OPND, bool BATCH>
 __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, uint8_t *b_base, TcShared *sh, float *exch) {
   constexpr int NJ = NT / 8;
   const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -81,178 +104,187 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   float *slot = exch + 256;  // fused statistics: per-warp partial sums [8 warps][2][128], fixed summation order
   float acc[NT / 2];
   uint32_t sa = 0, aph = 0, sb = 0, bph = 0, tl = 0;
-  for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x, ++tl) {
-    if (job.b_resident) sb = 0;
-    uint32_t scale = 0;
-    // one chunk of wgmmas stays in flight while the next is issued: a weight slot is released once the following chunk
-    // is committed and the slot's own chunk has completed, a patch stage once the last chunk that read it has completed
-    uint32_t b_prev = 0, a_prev = 0;
-    for (int g = 0; g < ngroups; ++g) {
-      mbar_wait(&sh->a_full[sa], aph);
-      // A descriptor start: pixel r of the patch is at +16 B * r, this warpgroup's rows begin 64 pixels in
-      const uint32_t a_hi16 = (smem_u32(a_base + sa * 2 * a_stage_bytes) >> 4) + (uint32_t)wg * 64u, a_lo16 = a_hi16 + a_stage16;
-      uint32_t sidx = 0;
-      for (int c = 0; c < nchunks; ++c) {
-        if (!job.b_resident || tl == 0) mbar_wait(&sh->b_full[sb], job.b_resident ? 0u : bph);
-        const uint32_t bh = (smem_u32(b_base + sb * chunk_bytes) >> 4) | ((uint32_t)NT << 16);  // LBO = Npad rows
-        wgmma_fence();
-        uint32_t bs = bh;
-        for (int st = 0; st < spc; ++st, bs += b_step16) {
-          const uint32_t dls = steps32[sidx + st];  // a_off16 | lbo16 << 16 (conv.cuh KStep)
-          const uint64_t ad_hi = kDescHi | (a_hi16 + dls), ad_lo = kDescHi | (a_lo16 + dls);
-          const uint64_t bd_hi = kDescHi | bs, bd_lo = kDescHi | (bs + b_lo16);
-          Wgmma<NT>::mma(acc, ad_hi, bd_hi, scale);
-          Wgmma<NT>::mma(acc, ad_lo, bd_hi, 1u);
-          Wgmma<NT>::mma(acc, ad_hi, bd_lo, 1u);
-          scale = 1;
-        }
-        wgmma_commit();
-        wgmma_wait<1>();  // every chunk but this one has completed
-        if ((g | c) && wt == 0) {
-          if (!job.b_resident) mbar_arrive(&sh->b_empty[b_prev]);
-          if (c == 0) mbar_arrive(&sh->a_empty[a_prev]);
-        }
-        b_prev = sb;
-        sidx += (uint32_t)spc;
-        if (++sb == nslots) { sb = 0; bph ^= 1; }
-      }
-      a_prev = sa;
-      if (++sa == nstages) { sa = 0; aph ^= 1; }
-    }
-    wgmma_wait<0>();
-    if (wt == 0) {
-      if (!job.b_resident) mbar_arrive(&sh->b_empty[b_prev]);
-      mbar_arrive(&sh->a_empty[a_prev]);
-    }
-    if (job.dbg & 8) continue;
-
-    // ===== epilogue from registers: acc[4i + 2h + e] = (pixel r0 + 8h, column 8i + q2 + e) =====
-    const int yu = tile / job.tiles_x, x0 = (tile - yu * job.tiles_x) * job.tile_dx;
-    const int y = yu, yo = y * job.oy_mul + job.oy_off;
-    if (job.xfold_kw) {
-      // partial sums Q[pixel][kx*Cout + co] -> shared memory, then out[x][co] = sum_kx Q[x + kx][kx*Cout + co]
-      const int ncol = job.xfold_kw * job.Cout;
-#pragma unroll
-      for (int i = 0; i < NJ; ++i)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int col = 8 * i + q2 + e;
-            if (col < ncol) exch[(r0 + 8 * h) * kExchPitch + col] = acc[4 * i + 2 * h + e];
+  const int total = (BATCH ? job.nimg : 1) * job.ntiles;
+  for (int tile = blockIdx.x; tile < total;) {
+    // this CTA's tiles of one image (tile_at), then that image's fused statistics: a CTA's tiles can cross into the next image, so
+    // the slot partials go out (and are cleared) before the next image's tiles add to them -- each image gets the per-CTA sums it
+    // gets when it runs alone (DESIGN.md 4.1)
+    const TileAt img = tile_at(job, tile, BATCH);
+    const int img_end = min(total, (img.b + 1) * job.ntiles);
+    for (; tile < img_end; tile += gridDim.x, ++tl) {
+      if (job.b_resident) sb = 0;
+      uint32_t scale = 0;
+      // one chunk of wgmmas stays in flight while the next is issued: a weight slot is released once the following chunk
+      // is committed and the slot's own chunk has completed, a patch stage once the last chunk that read it has completed
+      uint32_t b_prev = 0, a_prev = 0;
+      for (int g = 0; g < ngroups; ++g) {
+        mbar_wait(&sh->a_full[sa], aph);
+        // A descriptor start: pixel r of the patch is at +16 B * r, this warpgroup's rows begin 64 pixels in
+        const uint32_t a_hi16 = (smem_u32(a_base + sa * 2 * a_stage_bytes) >> 4) + (uint32_t)wg * 64u, a_lo16 = a_hi16 + a_stage16;
+        uint32_t sidx = 0;
+        for (int c = 0; c < nchunks; ++c) {
+          if (!job.b_resident || tl == 0) mbar_wait(&sh->b_full[sb], job.b_resident ? 0u : bph);
+          const uint32_t bh = (smem_u32(b_base + sb * chunk_bytes) >> 4) | ((uint32_t)NT << 16);  // LBO = Npad rows
+          wgmma_fence();
+          uint32_t bs = bh;
+          for (int st = 0; st < spc; ++st, bs += b_step16) {
+            const uint32_t dls = steps32[sidx + st];  // a_off16 | lbo16 << 16 (conv.cuh KStep)
+            const uint64_t ad_hi = kDescHi | (a_hi16 + dls), ad_lo = kDescHi | (a_lo16 + dls);
+            const uint64_t bd_hi = kDescHi | bs, bd_lo = kDescHi | (bs + b_lo16);
+            Wgmma<NT>::mma(acc, ad_hi, bd_hi, scale);
+            Wgmma<NT>::mma(acc, ad_lo, bd_hi, 1u);
+            Wgmma<NT>::mma(acc, ad_hi, bd_lo, 1u);
+            scale = 1;
           }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      const int px = threadIdx.x, x = x0 + px;
-      if (px < job.tile_dx && x < job.Wo && y < job.Ho && !(job.dbg & 1)) {
-        const int xo = x * job.ox_mul + job.ox_off;
-        const float *qv = exch + px * kExchPitch;
-        const int64_t plane = (int64_t)job.Ho * job.Wo, o = (int64_t)yo * job.Wo + xo;
-        for (int k = 0; k < job.Cout; ++k) {
-          float sum = __ldg(job.bias + k);
-          for (int kx = 0; kx < job.xfold_kw; ++kx) sum += qv[kx * (kExchPitch + job.Cout) + k];
-          job.out3[(job.final_mode == 2 ? 2 - k : k) * plane + o] = tc_final_value(sum, k, job.final_mode, job.tanh_c);
+          wgmma_commit();
+          wgmma_wait<1>();  // every chunk but this one has completed
+          if ((g | c) && wt == 0) {
+            if (!job.b_resident) mbar_arrive(&sh->b_empty[b_prev]);
+            if (c == 0) mbar_arrive(&sh->a_empty[a_prev]);
+          }
+          b_prev = sb;
+          sidx += (uint32_t)spc;
+          if (++sb == nslots) { sb = 0; bph ^= 1; }
         }
+        a_prev = sa;
+        if (++sa == nstages) { sa = 0; aph ^= 1; }
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");  // exch is rewritten by the next tile
-      continue;
-    }
-    bool valid[2];
-    int xo[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int x = x0 + r0 + 8 * h;
-      valid[h] = x < job.Wo && y < job.Ho && !(job.dbg & 1);
-      xo[h] = x * job.ox_mul + job.ox_off;
-    }
-    if (job.final_mode) {
-      // Cout <= 3 output channels sit in column group 0
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int k = q2 + e;
-          if (k < 3 && k < job.Cout && valid[h])
-            job.out3[((int64_t)(job.final_mode == 2 ? 2 - k : k) * job.Ho + yo) * job.Wo + xo[h]] =
-                tc_final_value(acc[2 * h + e] + __ldg(job.bias + k), k, job.final_mode, job.tanh_c);
+      wgmma_wait<0>();
+      if (wt == 0) {
+        if (!job.b_resident) mbar_arrive(&sh->b_empty[b_prev]);
+        mbar_arrive(&sh->a_empty[a_prev]);
+      }
+      if (job.dbg & 8) continue;
+
+      // ===== epilogue from registers: acc[4i + 2h + e] = (pixel r0 + 8h, column 8i + q2 + e) =====
+      const TileAt at = tile_at(job, tile, BATCH);  // y, x0; the image's offsets are img's
+      const int x0 = at.x0, y = at.y, yo = y * job.oy_mul + job.oy_off;
+      if (job.xfold_kw) {
+        // partial sums Q[pixel][kx*Cout + co] -> shared memory, then out[x][co] = sum_kx Q[x + kx][kx*Cout + co]
+        const int ncol = job.xfold_kw * job.Cout;
+  #pragma unroll
+        for (int i = 0; i < NJ; ++i)
+  #pragma unroll
+          for (int h = 0; h < 2; ++h)
+  #pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = 8 * i + q2 + e;
+              if (col < ncol) exch[(r0 + 8 * h) * kExchPitch + col] = acc[4 * i + 2 * h + e];
+            }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        const int px = threadIdx.x, x = x0 + px;
+        if (px < job.tile_dx && x < job.Wo && y < job.Ho && !(job.dbg & 1)) {
+          const int xo = x * job.ox_mul + job.ox_off;
+          const float *qv = exch + px * kExchPitch;
+          const int64_t plane = (int64_t)job.Ho * job.Wo, o = (int64_t)yo * job.Wo + xo;
+          for (int k = 0; k < job.Cout; ++k) {
+            float sum = __ldg(job.bias + k);
+            for (int kx = 0; kx < job.xfold_kw; ++kx) sum += qv[kx * (kExchPitch + job.Cout) + k];
+            job.out3[img.out3 + (job.final_mode == 2 ? 2 - k : k) * plane + o] = tc_final_value(sum, k, job.final_mode, job.tanh_c);
+          }
         }
-      continue;
-    }
-    if constexpr (OPND) {
-      // the two channels c, c + 1 of each of the thread's two pixels: BN scale and bias (+ReLU) (+skip) -> fp16 hi / lo pair, one 4-byte store
-      // per plane; the 4 lanes of a quad fill one 16-byte (pixel, channel block) cell.  No statistics, no atomics.
-      uint32_t *dhi = reinterpret_cast<uint32_t *>(job.epi_dst.hi), *dlo = reinterpret_cast<uint32_t *>(job.epi_dst.lo);
-#pragma unroll
+        asm volatile("bar.sync 1, 256;" ::: "memory");  // exch is rewritten by the next tile
+        continue;
+      }
+      bool valid[2];
+      int xo[2];
+  #pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int x = x0 + r0 + 8 * h;
+        valid[h] = x < job.Wo && y < job.Ho && !(job.dbg & 1);
+        xo[h] = x * job.ox_mul + job.ox_off;
+      }
+      if (job.final_mode) {
+        // Cout <= 3 output channels sit in column group 0
+  #pragma unroll
+        for (int h = 0; h < 2; ++h)
+  #pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int k = q2 + e;
+            if (k < 3 && k < job.Cout && valid[h])
+              job.out3[img.out3 + ((int64_t)(job.final_mode == 2 ? 2 - k : k) * job.Ho + yo) * job.Wo + xo[h]] =
+                  tc_final_value(acc[2 * h + e] + __ldg(job.bias + k), k, job.final_mode, job.tanh_c);
+          }
+        continue;
+      }
+      if constexpr (OPND) {
+        // the two channels c, c + 1 of each of the thread's two pixels: BN scale and bias (+ReLU) (+skip) -> fp16 hi / lo pair, one 4-byte store
+        // per plane; the 4 lanes of a quad fill one 16-byte (pixel, channel block) cell.  No statistics, no atomics.
+        uint32_t *dhi = reinterpret_cast<uint32_t *>(job.epi_dst.hi), *dlo = reinterpret_cast<uint32_t *>(job.epi_dst.lo);
+  #pragma unroll
+        for (int i = 0; i < NJ; ++i) {
+          const int c = 8 * i + q2;
+          // bias and scale are padded to Npad
+          const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c)), s = __ldg(reinterpret_cast<const float2 *>(job.epi_scale + c));
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            int64_t o, so;
+            // (a single image decodes the tile per store, as the register allocation of the unbatched kernel prefers)
+            if (!(BATCH ? opnd_epi_addr(job, at, threadIdx.x, i, h, o, so) : opnd_epi_addr(job, tile, threadIdx.x, i, h, o, so, false)))
+              continue;
+            float v0 = fmaf(acc[4 * i + 2 * h], s.x, b.x), v1 = fmaf(acc[4 * i + 2 * h + 1], s.y, b.y);
+            if (job.epi_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (job.epi_skip) {  // ConcatTable{conv_block, ShaveImage / Identity} -> CAddTable; same arithmetic as in_apply
+              const uint32_t sh = __ldg(reinterpret_cast<const uint32_t *>(job.epi_skip_op.hi) + so);
+              const uint32_t sl = __ldg(reinterpret_cast<const uint32_t *>(job.epi_skip_op.lo) + so);
+              const float2 fh = __half22float2(*reinterpret_cast<const __half2 *>(&sh));
+              const float2 fl = __half22float2(*reinterpret_cast<const __half2 *>(&sl));
+              v0 += fh.x + fl.x; v1 += fh.y + fl.y;
+            }
+            uint32_t hw, lw;
+            split_pair(v0, v1, hw, lw);
+            dhi[o] = hw; dlo[o] = lw;
+          }
+        }
+        continue;
+      }
+      const bool stats = job.stats && !(job.dbg & 64);
+      float *raw = job.raw + img.raw;
+  #pragma unroll
       for (int i = 0; i < NJ; ++i) {
         const int c = 8 * i + q2;
-        // bias and scale are padded to Npad
-        const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c)), s = __ldg(reinterpret_cast<const float2 *>(job.epi_scale + c));
-#pragma unroll
+        const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c));
+        float v[4];
+  #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          int64_t o, so;
-          if (!opnd_epi_addr(job, tile, threadIdx.x, i, h, o, so)) continue;
-          float v0 = fmaf(acc[4 * i + 2 * h], s.x, b.x), v1 = fmaf(acc[4 * i + 2 * h + 1], s.y, b.y);
-          if (job.epi_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-          if (job.epi_skip) {  // ConcatTable{conv_block, ShaveImage / Identity} -> CAddTable; same arithmetic as in_apply
-            const uint32_t sh = __ldg(reinterpret_cast<const uint32_t *>(job.epi_skip_op.hi) + so);
-            const uint32_t sl = __ldg(reinterpret_cast<const uint32_t *>(job.epi_skip_op.lo) + so);
-            const float2 fh = __half22float2(*reinterpret_cast<const __half2 *>(&sh));
-            const float2 fl = __half22float2(*reinterpret_cast<const __half2 *>(&sl));
-            v0 += fh.x + fl.x; v1 += fh.y + fl.y;
+          v[2 * h] = acc[4 * i + 2 * h] + b.x;
+          v[2 * h + 1] = acc[4 * i + 2 * h + 1] + b.y;
+          // raw layout [Ho][Cq][Wp][4]: channels c, c + 1 of one pixel are 8 contiguous bytes
+          if (valid[h] && c < job.Cout)
+            *reinterpret_cast<float2 *>(raw + (((int64_t)yo * job.raw_Cq + (c >> 2)) * job.raw_Wp + xo[h]) * 4 + (c & 3)) =
+                make_float2(v[2 * h], v[2 * h + 1]);
+          if (!valid[h]) v[2 * h] = v[2 * h + 1] = 0.f;
+        }
+        if (stats) {
+          // per-channel sums over the warp's 16 pixels: reduce over the 8 lanes that share lane % 4
+          float s0 = v[0] + v[2], s1 = v[1] + v[3], t0 = v[0] * v[0] + v[2] * v[2], t1 = v[1] * v[1] + v[3] * v[3];
+  #pragma unroll
+          for (int m = 4; m < 32; m <<= 1) {
+            s0 += __shfl_xor_sync(0xffffffffu, s0, m); s1 += __shfl_xor_sync(0xffffffffu, s1, m);
+            t0 += __shfl_xor_sync(0xffffffffu, t0, m); t1 += __shfl_xor_sync(0xffffffffu, t1, m);
           }
-          uint32_t hw, lw;
-          split_pair(v0, v1, hw, lw);
-          dhi[o] = hw; dlo[o] = lw;
-        }
-      }
-      continue;
-    }
-    const bool stats = job.stats && !(job.dbg & 64);
-#pragma unroll
-    for (int i = 0; i < NJ; ++i) {
-      const int c = 8 * i + q2;
-      const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c));
-      float v[4];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        v[2 * h] = acc[4 * i + 2 * h] + b.x;
-        v[2 * h + 1] = acc[4 * i + 2 * h + 1] + b.y;
-        // raw layout [Ho][Cq][Wp][4]: channels c, c + 1 of one pixel are 8 contiguous bytes
-        if (valid[h] && c < job.Cout)
-          *reinterpret_cast<float2 *>(job.raw + (((int64_t)yo * job.raw_Cq + (c >> 2)) * job.raw_Wp + xo[h]) * 4 + (c & 3)) =
-              make_float2(v[2 * h], v[2 * h + 1]);
-        if (!valid[h]) v[2 * h] = v[2 * h + 1] = 0.f;
-      }
-      if (stats) {
-        // per-channel sums over the warp's 16 pixels: reduce over the 8 lanes that share lane % 4
-        float s0 = v[0] + v[2], s1 = v[1] + v[3], t0 = v[0] * v[0] + v[2] * v[2], t1 = v[1] * v[1] + v[3] * v[3];
-#pragma unroll
-        for (int m = 4; m < 32; m <<= 1) {
-          s0 += __shfl_xor_sync(0xffffffffu, s0, m); s1 += __shfl_xor_sync(0xffffffffu, s1, m);
-          t0 += __shfl_xor_sync(0xffffffffu, t0, m); t1 += __shfl_xor_sync(0xffffffffu, t1, m);
-        }
-        if (lane < 4) {  // one writer per (warp, channel): deterministic
-          float *sl = slot + warp * 256;
-          sl[c] += s0; sl[c + 1] += s1; sl[128 + c] += t0; sl[128 + c + 1] += t1;
+          if (lane < 4) {  // one writer per (warp, channel): deterministic
+            float *sl = slot + warp * 256;
+            sl[c] += s0; sl[c + 1] += s1; sl[128 + c] += t0; sl[128 + c + 1] += t1;
+          }
         }
       }
     }
-  }
-  if (job.stats) {
-    // 8 warps' partial sums added in a FIXED order (deterministic per CTA: the tile -> CTA assignment is static), then one
-    // double atomic per channel and quantity per CTA
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const int ch = threadIdx.x;
-    if (ch < job.Cout) {
-      float ssum = 0.f, qsum = 0.f;
-#pragma unroll
-      for (int w = 0; w < 8; ++w) { ssum += slot[w * 256 + ch]; qsum += slot[w * 256 + 128 + ch]; }
-      atomicAdd(job.stats + ch, (double)ssum);
-      atomicAdd(job.stats + job.stats_pitch + ch, (double)qsum);
-    }
+    if (!OPND && job.stats) tc_flush_stats(job, slot, img.b, tile < total);  // an operand epilogue has no statistics
   }
 }
 
-template <int NT, bool OPND>
+// norm-on-load table of image b (threads tid, tid + nthr, ...)
+__device__ __forceinline__ void nl_build_table(const ConvJob &job, float *nl_tab, int b, int tid, int nthr) {
+  const double *sums = job.nl_sums + b * job.nl_sums_img;
+#pragma unroll 1  // kept rolled: an unrolled copy inside the producer loop costs the OPND instances a 4-byte spill
+  for (int c = tid; c < job.nl_C; c += nthr) {
+    in_finalize(sums[c], sums[job.nl_C + c], job.nl_inv_count, job.nl_eps, job.nl_gamma[c], nl_tab[c], nl_tab[kNlMaxC + c]);
+    nl_tab[2 * kNlMaxC + c] = job.nl_beta[c];
+  }
+}
+
+template <int NT, bool OPND, bool BATCH>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ ConvJob job) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t a_stage_bytes = (uint32_t)job.stage16 * 16u;  // one of hi / lo
@@ -281,18 +313,16 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   // norm-on-load: mean / gamma*rstd / beta per input channel from the producer conv's fused statistics (same arithmetic
   // as in_apply_kernel: biased variance, eps inside the sqrt, InstanceNormalization.lua:39-50)
   float *nl_tab = exch + (256 + 8 * 2 * 128);
-  if (job.nl)
-    for (int c = threadIdx.x; c < job.nl_C; c += blockDim.x) {
-      in_finalize(job.nl_sums[c], job.nl_sums[job.nl_C + c], job.nl_inv_count, job.nl_eps, job.nl_gamma[c], nl_tab[c], nl_tab[kNlMaxC + c]);
-      nl_tab[2 * kNlMaxC + c] = job.nl_beta[c];
-    }
+  const int total = (BATCH ? job.nimg : 1) * job.ntiles;
+  int nl_b = BATCH ? (int)blockIdx.x / job.ntiles : 0;  // image whose statistics nl_tab holds
+  if (job.nl) nl_build_table(job, nl_tab, nl_b, threadIdx.x, blockDim.x);
   __syncthreads();
   if (threadIdx.x == 0 && job.trace) trace_put(job, 2, clock64());
 
   const int ngroups = job.ngroups, nchunks = job.nchunks;
 
   if (warp < 8) {
-    tc_consume<NT, OPND>(job, a_base, b_base, sh, exch);
+    tc_consume<NT, OPND, BATCH>(job, a_base, b_base, sh, exch);
   } else if (job.nl && warp >= kAWarp) {
     // ===== norm-on-load patch producers: raw fp32 -> InstanceNorm (+ReLU) -> fp16 hi/lo -> MMA-ready stage =====
     // A warp owns whole (patch row, channel block) slabs: lanes run along x (coalesced 512-byte loads), up to
@@ -300,10 +330,18 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     const int pw = warp - kAWarp;
     const int pslab = job.pslab16, nslabs = job.nrows * job.CbG;
     uint32_t s = 0, ph = 0;
-    for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) {
-      const int yu = tile / job.tiles_x, x0 = (tile - yu * job.tiles_x) * job.tile_dx;
-      const int y = yu;
-      const int xb = job.seg_src16[0] + x0 - job.nl_padL;  // raw column of patch pixel 0
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      const TileAt at = tile_at(job, tile, BATCH);
+      const int y = at.y;
+      const int xb = job.seg_src16[0] + at.x0 - job.nl_padL;  // raw column of patch pixel 0
+      if (at.b != nl_b) {
+        // the next image: its table replaces the current one once all four producer warps are done with the previous tile
+        nl_b = at.b;
+        asm volatile("bar.sync 2, 128;" ::: "memory");
+        nl_build_table(job, nl_tab, nl_b, threadIdx.x - kAWarp * 32, 32 * kNlWarps);
+        asm volatile("bar.sync 2, 128;" ::: "memory");
+      }
+      const float4 *nl_raw = job.nl_raw + at.nl_raw4;
       for (int g = 0; g < ngroups; ++g) {
         mbar_wait(&sh->a_empty[s], ph ^ 1);
         uint8_t *stage = a_base + s * 2 * a_stage_bytes;
@@ -311,7 +349,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
           const int ri = rc / job.CbG, cbi = rc - ri * job.CbG;
           const int ry = job.row_mul * y + job.grp_row[g][ri] - job.nl_padT, cb = job.grp_cb0[g] + cbi;
           const bool row_ok = ry >= 0 && ry < job.nl_H;
-          const float4 *rp = job.nl_raw + ((int64_t)(row_ok ? ry : 0) * job.nl_Cq + 2 * cb) * job.nl_Wp;
+          const float4 *rp = nl_raw + ((int64_t)(row_ok ? ry : 0) * job.nl_Cq + 2 * cb) * job.nl_Wp;
           float tm[8], ts[8], tb[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) { tm[i] = nl_tab[cb * 8 + i]; ts[i] = nl_tab[kNlMaxC + cb * 8 + i]; tb[i] = nl_tab[2 * kNlMaxC + cb * 8 + i]; }
@@ -366,9 +404,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     for (int s = 0; s < job.nseg; ++s) stage_tx += (job.dbg & 4) ? 16u : (uint32_t)job.seg_len16[s] * 16u;
     stage_tx *= (uint32_t)(job.nrows * job.CbG * 2);
     uint32_t s = 0, ph = 0;
-    for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) {
-      const int yu = tile / job.tiles_x, x0 = (tile - yu * job.tiles_x) * job.tile_dx;
-      const int y = yu;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      const TileAt at = tile_at(job, tile, BATCH);
+      const int y = at.y, x0 = at.x0;
       for (int g = 0; g < ngroups; ++g) {
         mbar_wait(&sh->a_empty[s], ph ^ 1);
         if (lane == 0) mbar_arrive_expect_tx(&sh->a_full[s], stage_tx);
@@ -380,7 +418,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
           r -= cbi * job.nseg * 2;
           int seg = r >> 1, part = r & 1;
           int64_t src16 = ((int64_t)(job.row_mul * y + job.grp_row[g][ri]) * job.a_Cb + job.grp_cb0[g] + cbi) *
-                              job.a_slab16 + job.seg_src16[seg] + x0;
+                              job.a_slab16 + job.seg_src16[seg] + x0 + at.a16;
           const uint4 *src = (part ? job.a_lo : job.a_hi) + src16;
           uint8_t *dst = stage + part * a_stage_bytes +
                          (uint32_t)((ri * job.CbG + cbi) * job.pslab16 + job.seg_dst16[seg]) * 16u;
@@ -393,7 +431,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     // ===== B producer: weight chunks =====
     if (lane == 0) {
       uint32_t s = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
         if (job.b_resident && tile != (int)blockIdx.x) break;  // resident weights: one pass fills every slot
         for (int g = 0; g < ngroups; ++g)
           for (int c = 0; c < nchunks; ++c) {
@@ -412,7 +450,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   if (threadIdx.x == 0 && job.trace) {
     trace_put(job, 3, clock64());
     int nu = 0;
-    for (int tile = blockIdx.x; tile < job.ntiles; tile += gridDim.x) ++nu;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) ++nu;
     trace_put(job, 4, nu);
   }
 }
@@ -473,7 +511,12 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
     return FAV_ERR_UNSUPPORTED;
   }
   void (*kernel)(ConvJob) = nullptr;
-#define FAV_TC_CASE(N) case N: kernel = job.opnd ? conv_tc_kernel<N, true> : conv_tc_kernel<N, false>; break;
+  const bool batch = job.nimg > 1;
+#define FAV_TC_CASE(N)                                                                                         \
+  case N:                                                                                                      \
+    kernel = job.opnd ? (batch ? conv_tc_kernel<N, true, true> : conv_tc_kernel<N, true, false>)              \
+                      : (batch ? conv_tc_kernel<N, false, true> : conv_tc_kernel<N, false, false>);           \
+    break;
   switch (job.Npad) {
     FAV_TC_CASE(16) FAV_TC_CASE(32) FAV_TC_CASE(48) FAV_TC_CASE(64) FAV_TC_CASE(80) FAV_TC_CASE(96) FAV_TC_CASE(112)
     FAV_TC_CASE(128)
@@ -482,24 +525,25 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
       return FAV_ERR_UNSUPPORTED;
   }
 #undef FAV_TC_CASE
-  job.trace = conv_trace_claim((size_t)(job.ntiles < num_sms ? job.ntiles : num_sms) * kTraceWords);
+  // one persistent CTA per SM over the tiles of every image (tile_at); the grid of a single image is unchanged
+  const int total = job.nimg * job.ntiles, grid = total < num_sms ? total : num_sms;
+  job.trace = conv_trace_claim((size_t)grid * kTraceWords);
   size_t smem = conv_tc_smem_bytes(job);
   if (smem > 227 * 1024) {
     set_error("conv_tc: shared memory %zu exceeds 227 KB", smem);
     return FAV_ERR_UNSUPPORTED;
   }
   // the opt-in to > 48 KB of dynamic shared memory is a PER-DEVICE attribute of each instantiation
-  static std::atomic<uint64_t> attr_set[18];
+  static std::atomic<uint64_t> attr_set[36];
   int dev = 0;
   FAV_TRY(check_cuda(cudaGetDevice(&dev), "cudaGetDevice"));
   const uint64_t bit = 1ull << (dev & 63);
-  std::atomic<uint64_t> &set = attr_set[job.Npad / 16 + (job.opnd ? 9 : 0)];
+  std::atomic<uint64_t> &set = attr_set[job.Npad / 16 + (job.opnd ? 9 : 0) + (batch ? 18 : 0)];
   if (!(set.load(std::memory_order_acquire) & bit)) {
     FAV_TRY(check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
                        "cudaFuncSetAttribute(conv_tc)"));
     set.fetch_or(bit, std::memory_order_release);
   }
-  const int grid = job.ntiles < num_sms ? job.ntiles : num_sms;
   kernel<<<grid, job.nl ? kThreads : kConsumerThreads + 64, smem, st>>>(job);
   return post_launch("conv_tc");
 }

@@ -306,6 +306,10 @@ __device__ __forceinline__ void temporal_pixels(
   }
 }
 
+// a batch of images (blockIdx.z = image b): every plane argument holds one image after the other, dst is image b of the operand
+template <class T>
+__device__ __forceinline__ T *img_plane(T *p, int b, int64_t per_image) { return p ? p + b * per_image : p; }
+
 template <int VEC, bool FIRST, bool PACK = false>
 __global__ void __launch_bounds__(256) temporal_input_kernel(
     const float *__restrict__ content, const float *__restrict__ prev, const float *__restrict__ flow,
@@ -314,6 +318,13 @@ __global__ void __launch_bounds__(256) temporal_input_kernel(
   int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * VEC;
   int y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x0 >= W || y >= H) return;
+  if (const int b = blockIdx.z) {
+    const int64_t HW = (int64_t)H * W;
+    content = img_plane(content, b, 3 * HW); prev = img_plane(prev, b, 3 * HW); flow = img_plane(flow, b, 2 * HW);
+    cert = img_plane(cert, b, HW); fill = img_plane(fill, b, 3 * HW); flow_mask = img_plane(flow_mask, b, HW);
+    out7 = img_plane(out7, b, 7 * HW);
+    dst = image_of(dst, b);
+  }
   const int64_t o = (int64_t)y * W + x0;
   float c[VEC];
   if (!FIRST) {
@@ -352,6 +363,13 @@ __global__ void __launch_bounds__(256) temporal_stage_kernel(
   const int p = r / 2, bx = blockIdx.x * TS_TX, by = blockIdx.y * TS_TY;
   const int tw = TS_TX + 2 * p, th = TS_TY + 2 * p;
   const int64_t HW = (int64_t)H * W;
+  if (const int b = blockIdx.z) {  // a batch: image b of every plane (img_plane) and of the operand
+    content = img_plane(content, b, 3 * HW); prev = img_plane(prev, b, 3 * HW); flow = img_plane(flow, b, 2 * HW);
+    fw_u = img_plane(fw_u, b, 2 * HW); fw_v = img_plane(fw_v, b, 2 * HW); cert_raw = img_plane(cert_raw, b, HW);
+    fill = img_plane(fill, b, 3 * HW); flow_mask = img_plane(flow_mask, b, HW); out7 = img_plane(out7, b, 7 * HW);
+    cert_out = img_plane(cert_out, b, HW);
+    dst = image_of(dst, b);
+  }
   if (MODE == 0) {
     // kTsBatch pixels per thread and pass: first the (coalesced) backward-flow loads of all of them, then all their forward-flow
     // gathers, then the arithmetic -- up to 8 * kTsBatch loads in flight per thread instead of one pixel's dependent chain
@@ -431,18 +449,18 @@ __global__ void __launch_bounds__(256) temporal_stage_kernel(
 // run_[next_]image: the fused input written straight into the first operand of the network (no out7 round trip)
 int launch_temporal_input_packed(const float *content, const float *prev, const float *flow, const float *cert,
                                  const float *fill, const float *flow_mask, const Operand &dst, int R, int H, int W,
-                                 int border_mode, bool first, cudaStream_t st) {
+                                 int border_mode, bool first, cudaStream_t st, int nimg = 1) {
   const bool vec = (W % 4 == 0) && aligned16(content) && (first || (aligned16(flow) && aligned16(cert))) &&
                    (!flow_mask || aligned16(flow_mask)) && (!fill || aligned16(fill));
   dim3 block(32, 8);
   if (vec) {
-    dim3 grid(ceil_div(W / 4, 32), ceil_div(H, 8));
+    dim3 grid(ceil_div(W / 4, 32), ceil_div(H, 8), nimg);
     if (first)
       temporal_input_kernel<4, true, true><<<grid, block, 0, st>>>(content, prev, flow, cert, fill, flow_mask, nullptr, H, W, border_mode, dst, R);
     else
       temporal_input_kernel<4, false, true><<<grid, block, 0, st>>>(content, prev, flow, cert, fill, flow_mask, nullptr, H, W, border_mode, dst, R);
   } else {
-    dim3 grid(ceil_div(W, 32), ceil_div(H, 8));
+    dim3 grid(ceil_div(W, 32), ceil_div(H, 8), nimg);
     if (first)
       temporal_input_kernel<1, true, true><<<grid, block, 0, st>>>(content, prev, flow, cert, fill, flow_mask, nullptr, H, W, border_mode, dst, R);
     else
@@ -456,12 +474,12 @@ int launch_temporal_input_packed(const float *content, const float *prev, const 
 // (callers then fall back to the three separate kernels).
 int launch_temporal_stage(const float *content, const float *prev, const float *flow, const float *fw_uv, const float *cert_raw,
                           const float *fill, const float *flow_mask, float *out7, float *cert_out, const Operand *dst, int R,
-                          int H, int W, int r, int border_mode, cudaStream_t st) {
+                          int H, int W, int r, int border_mode, cudaStream_t st, int nimg = 1) {
   const bool vec = (W % 4 == 0) && aligned16(content) && aligned16(flow) && (!flow_mask || aligned16(flow_mask)) &&
                    (!fill || aligned16(fill)) && (!out7 || aligned16(out7)) && (!cert_out || aligned16(cert_out));
   if (!vec || r < 0 || r / 2 > TS_MAXP || (r > 1 && !(r & 1))) return FAV_ERR_UNSUPPORTED;
   const int64_t HW = (int64_t)H * W;
-  dim3 grid(ceil_div(W, TS_TX), ceil_div(H, TS_TY));
+  dim3 grid(ceil_div(W, TS_TX), ceil_div(H, TS_TY), nimg);
   const Operand d = dst ? *dst : Operand();
   if (fw_uv) {
     if (dst) temporal_stage_kernel<true, 0><<<grid, 256, 0, st>>>(content, prev, flow, fw_uv, fw_uv + HW, nullptr, fill, flow_mask, nullptr, cert_out, H, W, r, border_mode, d, R);
@@ -475,18 +493,18 @@ int launch_temporal_stage(const float *content, const float *prev, const float *
 
 int launch_temporal_input(const float *content, const float *prev, const float *flow, const float *cert,
                           const float *fill, const float *flow_mask, float *out7, int H, int W,
-                          int border_mode, bool first, cudaStream_t st) {
+                          int border_mode, bool first, cudaStream_t st, int nimg = 1) {
   bool vec = (W % 4 == 0) && aligned16(content) && aligned16(out7) && (first || (aligned16(flow) && aligned16(cert))) &&
              (!flow_mask || aligned16(flow_mask));
   dim3 block(32, 8);
   if (vec) {
-    dim3 grid(ceil_div(W / 4, 32), ceil_div(H, 8));
+    dim3 grid(ceil_div(W / 4, 32), ceil_div(H, 8), nimg);
     if (first)
       temporal_input_kernel<4, true><<<grid, block, 0, st>>>(content, prev, flow, cert, fill, flow_mask, out7, H, W, border_mode);
     else
       temporal_input_kernel<4, false><<<grid, block, 0, st>>>(content, prev, flow, cert, fill, flow_mask, out7, H, W, border_mode);
   } else {
-    dim3 grid(ceil_div(W, 32), ceil_div(H, 8));
+    dim3 grid(ceil_div(W, 32), ceil_div(H, 8), nimg);
     if (first)
       temporal_input_kernel<1, true><<<grid, block, 0, st>>>(content, prev, flow, cert, fill, flow_mask, out7, H, W, border_mode);
     else

@@ -8,6 +8,7 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <tuple>
 #include <vector>
 #include <cmath>
 #include <cstring>
@@ -18,16 +19,16 @@ namespace fav {
 
 int launch_temporal_input(const float *content, const float *prev, const float *flow, const float *cert,
                           const float *fill, const float *flow_mask, float *out7, int H, int W, int border_mode,
-                          bool first, cudaStream_t st);
+                          bool first, cudaStream_t st, int nimg = 1);
 int launch_temporal_stage(const float *content, const float *prev, const float *flow, const float *fw_uv, const float *cert_raw,
                           const float *fill, const float *flow_mask, float *out7, float *cert_out, const Operand *dst, int R,
-                          int H, int W, int r, int border_mode, cudaStream_t st);
+                          int H, int W, int r, int border_mode, cudaStream_t st, int nimg = 1);
 int launch_min_filter(const float *in, float *out, int n, int H, int W, int r, cudaStream_t st);
 int launch_consistency(const float *f1u, const float *f1v, const float *f2u, const float *f2v, const float *structure,
                        const float *avg_dev, float avg_host, uint8_t *rel, float *cert, int W, int H, cudaStream_t st);
 int launch_temporal_input_packed(const float *content, const float *prev, const float *flow, const float *cert,
                                  const float *fill, const float *flow_mask, const Operand &dst, int R, int H, int W,
-                                 int border_mode, bool first, cudaStream_t st);
+                                 int border_mode, bool first, cudaStream_t st, int nimg = 1);
 
 // ---------------------------------------------------------------------------------------------------------
 struct Param {
@@ -79,14 +80,21 @@ struct PlanStep {
   bool fused_nl = false; // kind 1: the tcgen05 consumer normalises on load (conv_tc.cu), this pass is skipped
 };
 
+// a batch: B frames of one size run through one plan, every kernel covering all B images in one launch (conv.cuh tile_at);
+// operands, raw tensors and statistics hold one image after the other, each with its own zero border
+constexpr int kMaxBatch = 64;
+constexpr size_t kMaxPlanBytes = (size_t)32 << 30;  // activation buffers of one plan, checked before each allocation
+
 struct Plan {
-  int H = 0, W = 0;
+  int B = 1, H = 0, W = 0;
+  size_t bytes = 0;        // device memory of the activation buffers (kMaxPlanBytes)
+  int64_t stats_img = 0;   // doubles of statistics per image
   std::vector<Operand> ops;
   std::vector<void *> allocs;
   float *raw_buf = nullptr, *raw_buf2 = nullptr;  // consecutive convolutions alternate (norm-on-load reads one, writes the other)
   size_t raw_bytes = 0;  // of each; a batch-normalized net allocates them only for the CUDA-core comparator (ensure_raw)
   double *stats = nullptr;
-  size_t stats_bytes = 0;
+  size_t stats_bytes = 0;  // all B images
   float *msb = nullptr;
   float *in7 = nullptr, *out3 = nullptr;  // scratch for run_image / run_next_image
   float *cert_a = nullptr, *cert_b = nullptr;  // scratch of the unfused fallback of fav_run_next_image_flows
@@ -124,7 +132,7 @@ struct fav_net {
   int num_sms = 148;
   cudaStream_t cap_stream = nullptr;  // graph capture happens here (the caller's stream may be the legacy default stream)
   int device = 0;
-  std::map<std::pair<int, int>, std::unique_ptr<Plan>> plans;
+  std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>> plans;  // (B, H, W)
   Plan *last_plan = nullptr;
   std::vector<void *> allocs;
   ~fav_net() {
@@ -280,6 +288,12 @@ static int fold_batch_norms(fav_net *net, std::vector<std::vector<float>> &w, st
 
 // ---- plan ---------------------------------------------------------------------------------------------------
 static int alloc_zero(Plan &pl, void **out, size_t bytes) {
+  pl.bytes += bytes;
+  if (pl.bytes > kMaxPlanBytes) {
+    set_error("a batch of %d frames of %dx%d needs more than %zu GiB of activations: use a smaller batch", pl.B, pl.W, pl.H,
+              kMaxPlanBytes >> 30);
+    return FAV_ERR_INVALID;
+  }
   FAV_TRY(check_cuda(cudaMalloc(out, bytes), "cudaMalloc(activations)"));
   pl.allocs.push_back(*out);
   return check_cuda(cudaMemset(*out, 0, bytes), "cudaMemset(activations)");
@@ -288,8 +302,9 @@ static int alloc_zero(Plan &pl, void **out, size_t bytes) {
 // operand feeding convolution `c` (its pad / parity requirements)
 static int make_operand(Plan &pl, int C, int H, int W, const ConvDef *consumer, int *index) {
   Operand o = operand_geometry(C, H, W, consumer);
-  FAV_TRY(alloc_zero(pl, (void **)&o.hi, o.elems16 * 16));
-  FAV_TRY(alloc_zero(pl, (void **)&o.lo, o.elems16 * 16));
+  o.img16 = (int64_t)o.elems16;
+  FAV_TRY(alloc_zero(pl, (void **)&o.hi, pl.B * o.elems16 * 16));
+  FAV_TRY(alloc_zero(pl, (void **)&o.lo, pl.B * o.elems16 * 16));
   pl.ops.push_back(o);
   *index = (int)pl.ops.size() - 1;
   return FAV_OK;
@@ -312,6 +327,7 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
       if (use_fold) {
         if (!fold_done) {
           FAV_TRY(fill_conv_job(cd, cd.fold, in, j));
+          set_conv_batch(j, pl.B, st.raw.img, 3ll * pl.H * pl.W, pl.stats_img);
           j.b = cd.fold.d_b_tc; j.bias = cd.d_bias;
           j.raw = raw; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
           j.final_mode = 0; j.out3 = out3; j.tanh_c = net->tanh_c;
@@ -324,6 +340,7 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
         }
       } else {
         FAV_TRY(fill_conv_job(cd, ph, in, j));
+        set_conv_batch(j, pl.B, st.raw.img, 3ll * pl.H * pl.W, pl.stats_img);
         j.b = ph.d_b_tc; j.bias = cd.d_bias;
         j.raw = raw; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
         j.final_mode = last ? 1 : 0; j.out3 = out3; j.tanh_c = net->tanh_c;
@@ -355,8 +372,12 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
   return FAV_OK;
 }
 
-static int build_plan(fav_net *net, int H, int W, Plan **out) {
-  auto key = std::make_pair(H, W);
+static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
+  if (B < 1 || B > kMaxBatch) {
+    set_error("batch of %d frames: 1 to %d frames per call", B, kMaxBatch);
+    return FAV_ERR_INVALID;
+  }
+  auto key = std::make_tuple(B, H, W);
   auto it = net->plans.find(key);
   if (it != net->plans.end()) { *out = it->second.get(); net->last_plan = *out; return FAV_OK; }
   if (H % 4 || W % 4 || H < 16 || W < 16) {
@@ -365,7 +386,7 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
     return FAV_ERR_INVALID;
   }
   std::unique_ptr<Plan> pl(new Plan());
-  pl->H = H; pl->W = W;
+  pl->B = B; pl->H = H; pl->W = W;
   const int R = net->reflect_pad;
   if (R >= H || R >= W) { set_error("frame smaller than the reflection padding (%d)", R); return FAV_ERR_INVALID; }
   // pass 1: sizes -> largest raw tensor, stats slots
@@ -386,16 +407,17 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       }
     }
   }
-  pl->raw_bytes = raw_max * sizeof(float) + 4096;
+  pl->raw_bytes = raw_max * sizeof(float) + 4096;  // per image (a multiple of 16 bytes)
   if (!net->bn) {  // a batch-normalized net's tensor-core epilogues write operands, not raw tensors
-    FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf, pl->raw_bytes));
-    FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf2, pl->raw_bytes));
+    FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf, B * pl->raw_bytes));
+    FAV_TRY(alloc_zero(*pl, (void **)&pl->raw_buf2, B * pl->raw_bytes));
   }
-  pl->stats_bytes = std::max(1, stats_slots) * sizeof(double);
+  pl->stats_img = std::max(1, stats_slots);
+  pl->stats_bytes = B * pl->stats_img * sizeof(double);
   FAV_TRY(alloc_zero(*pl, (void **)&pl->stats, pl->stats_bytes));
   FAV_TRY(alloc_zero(*pl, (void **)&pl->msb, std::max(1, stats_slots) * 2 * sizeof(float)));
-  FAV_TRY(alloc_zero(*pl, (void **)&pl->in7, (size_t)net->in_dim * H * W * sizeof(float)));
-  FAV_TRY(alloc_zero(*pl, (void **)&pl->out3, (size_t)3 * H * W * sizeof(float)));
+  FAV_TRY(alloc_zero(*pl, (void **)&pl->in7, (size_t)B * net->in_dim * H * W * sizeof(float)));
+  FAV_TRY(alloc_zero(*pl, (void **)&pl->out3, (size_t)B * 3 * H * W * sizeof(float)));
 
   // flat list of convs in execution order, to look up the consumer of each operand
   std::vector<int> order;
@@ -433,7 +455,7 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
       conv_out_size(c, pl->ops[cur].H, pl->ops[cur].W, &ho, &wo);
       cs.raw.p = (pos & 1) ? pl->raw_buf2 : pl->raw_buf; cs.raw_sel = (int)(pos & 1);
       cs.raw.C = c.cout; cs.raw.Cq = round_up(c.cout, 4) / 4; cs.raw.H = ho; cs.raw.W = wo;
-      cs.raw.Hp = ho + 2; cs.raw.Wp = round_up(wo, kTileM);
+      cs.raw.Hp = ho + 2; cs.raw.Wp = round_up(wo, kTileM); cs.raw.img = (int64_t)(pl->raw_bytes / sizeof(float));
       const bool last = op.last && i == n - 1;
       if (last) {
         FAV_TRY(build_conv_jobs(net, *pl, cs, c, true, nullptr, nullptr));
@@ -481,6 +503,7 @@ static int build_plan(fav_net *net, int H, int W, Plan **out) {
             t.nl_raw = reinterpret_cast<const float4 *>(ap.raw.p); t.nl_Cq = ap.raw.Cq; t.nl_Wp = ap.raw.Wp;
             t.nl_H = ap.raw.H; t.nl_W = ap.raw.W; t.nl_padT = in.padT; t.nl_padL = in.padL; t.nl_relu = ap.relu; t.nl_C = n.C;
             t.nl_sums = pl->stats + ap.stats_off; t.nl_gamma = n.d_gamma; t.nl_beta = n.d_beta;
+            t.nl_raw_img4 = ap.raw.img / 4; t.nl_sums_img = pl->stats_img;
             t.nl_inv_count = 1.0 / ((double)ap.raw.H * ap.raw.W); t.nl_eps = 1e-5;
             conv_tc_choose_slots(t);
             ok = conv_tc_smem_bytes(t) <= 227 * 1024 && (t.b_resident || t.b_slots >= 2);
@@ -512,8 +535,8 @@ struct ProfRec {
 // the raw tensors of a batch-normalized net, which only the CUDA-core comparator writes: allocated at its first run
 static int ensure_raw(Plan &pl) {
   if (pl.raw_buf) return FAV_OK;
-  FAV_TRY(alloc_zero(pl, (void **)&pl.raw_buf, pl.raw_bytes));
-  FAV_TRY(alloc_zero(pl, (void **)&pl.raw_buf2, pl.raw_bytes));
+  FAV_TRY(alloc_zero(pl, (void **)&pl.raw_buf, pl.B * pl.raw_bytes));
+  FAV_TRY(alloc_zero(pl, (void **)&pl.raw_buf2, pl.B * pl.raw_bytes));
   for (PlanStep &s : pl.steps) {
     float *p = s.raw_sel ? pl.raw_buf2 : pl.raw_buf;
     s.raw.p = p;
@@ -544,7 +567,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
   if (!net->bn) FAV_TRY(check_cuda(cudaMemsetAsync(pl.stats, 0, pl.stats_bytes, st), "cudaMemsetAsync(stats)"));
   if (in7) {
     FAV_TRY(begin(0, (double)pl.ops[0].H * pl.ops[0].W * (4.0 * net->in_dim + 32.0), "pack_input"));
-    FAV_TRY(launch_pack_input(in7, net->in_dim, pl.H, pl.W, net->reflect_pad, pl.ops[0], st));
+    FAV_TRY(launch_pack_input(in7, net->in_dim, pl.H, pl.W, net->reflect_pad, pl.ops[0], st, pl.B));
     FAV_TRY(end());
   }
   for (PlanStep &s : pl.steps) {
@@ -563,7 +586,13 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
       } else {
         for (SimtJob &j : s.simt) {
           if (j.final_mode) { j.final_mode = final_mode; j.out3 = out3; }
-          FAV_TRY(launch_conv_simt(j, st));
+          for (int b = 0; b < pl.B; ++b) {  // the comparator runs one image at a time
+            SimtJob jb = j;
+            jb.in = image_of(j.in, b);
+            jb.raw = j.raw ? j.raw + b * s.raw.img : nullptr;
+            jb.out3 = j.out3 ? j.out3 + (int64_t)b * 3 * pl.H * pl.W : nullptr;
+            FAV_TRY(launch_conv_simt(jb, st));
+          }
         }
       }
       FAV_TRY(end());
@@ -572,7 +601,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
       const Operand &src = pl.ops[s.src];
       FAV_TRY(begin(3, 12.0 * n.C * src.H * src.W * (1.0 + s.scale * s.scale) / 2.0, n.name + ".up"));
       FAV_TRY(launch_up_in(src, pl.stats + s.stats_off, n.d_gamma, n.d_beta, 1e-5f, s.relu, s.scale, pl.ops[s.dst], st, n.d_mean,
-                           n.d_scale));
+                           n.d_scale, pl.B, pl.stats_img));
       FAV_TRY(end());
     } else {
       if (s.fused_nl && net->conv_impl == 0) continue;  // the consumer conv normalises while it loads (norm-on-load)
@@ -581,7 +610,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
         if (net->conv_impl == 0) continue;
         FAV_TRY(begin(3, (s.skip >= 0 ? 12.0 : 8.0) * n.C * s.raw.H * s.raw.W, n.name + ".apply"));
         FAV_TRY(launch_in_apply(s.raw, nullptr, nullptr, nullptr, 0.f, s.relu, s.skip >= 0 ? &pl.ops[s.skip] : nullptr, s.shave,
-                                pl.ops[s.dst], st));
+                                pl.ops[s.dst], st, pl.B));
         FAV_TRY(end());
         continue;
       }
@@ -589,13 +618,13 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
       const double elems = (double)n.C * s.raw.H * s.raw.W;
       if (net->conv_impl != 0) {  // the tcgen05 epilogue already accumulated the statistics
         FAV_TRY(begin(2, 4.0 * elems, n.name + ".stats"));
-        FAV_TRY(launch_in_stats(s.raw, sums, st));
+        FAV_TRY(launch_in_stats(s.raw, sums, st, pl.B, pl.stats_img));
         FAV_TRY(end());
       }
       // InstanceNormalization.lua:21,39: eps = 1e-5, statistics over H*W of each (n, c)
       FAV_TRY(begin(3, (s.skip >= 0 ? 12.0 : 8.0) * elems, n.name + ".apply"));
       FAV_TRY(launch_in_apply(s.raw, sums, n.d_gamma, n.d_beta, 1e-5f, s.relu, s.skip >= 0 ? &pl.ops[s.skip] : nullptr, s.shave,
-                              pl.ops[s.dst], st));
+                              pl.ops[s.dst], st, pl.B, pl.stats_img));
       FAV_TRY(end());
     }
   }
@@ -836,11 +865,15 @@ int fav_net_set_conv_impl(fav_net_t *net, int impl) {
 }
 
 int fav_net_forward(fav_net_t *net, const float *in7, int H, int W, float *out3, void *stream) {
-  FAV_REQUIRE(net && in7 && out3, "fav_net_forward: null argument");
+  return fav_net_forward_batch(net, in7, 1, H, W, out3, stream);
+}
+
+int fav_net_forward_batch(fav_net_t *net, const float *in, int B, int H, int W, float *out3, void *stream) {
+  FAV_REQUIRE(net && in && out3, "fav_net_forward: null argument");
   FAV_REQUIRE(net->finalized, "fav_net_forward: call fav_net_finalize first");
   Plan *pl;
-  FAV_TRY(build_plan(net, H, W, &pl));
-  return run_plan(net, *pl, in7, out3, 1, (cudaStream_t)stream);
+  FAV_TRY(build_plan(net, B, H, W, &pl));
+  return run_plan(net, *pl, in, out3, 1, (cudaStream_t)stream);
 }
 
 int fav_net_profile(fav_net_t *net, const float *in7, int H, int W, float *out3, int max_steps, int *kinds, float *ms,
@@ -848,7 +881,7 @@ int fav_net_profile(fav_net_t *net, const float *in7, int H, int W, float *out3,
   FAV_REQUIRE(net && in7 && out3 && kinds && ms && work && n_out, "fav_net_profile: null argument");
   FAV_REQUIRE(net->finalized, "fav_net_profile: call fav_net_finalize first");
   Plan *pl;
-  FAV_TRY(build_plan(net, H, W, &pl));
+  FAV_TRY(build_plan(net, 1, H, W, &pl));
   std::vector<ProfRec> prof;
   cudaStream_t st = (cudaStream_t)stream;
   int rc = run_plan(net, *pl, in7, out3, 1, st, &prof);
@@ -869,8 +902,13 @@ int fav_net_profile(fav_net_t *net, const float *in7, int H, int W, float *out3,
 }
 
 int fav_net_layer_output(fav_net_t *net, int index, float *out, int *C, int *Hl, int *Wl, void *stream) {
+  return fav_net_layer_output_image(net, index, 0, out, C, Hl, Wl, stream);
+}
+
+int fav_net_layer_output_image(fav_net_t *net, int index, int b, float *out, int *C, int *Hl, int *Wl, void *stream) {
   FAV_REQUIRE(net && net->last_plan, "fav_net_layer_output: run a forward first");
   Plan *pl = net->last_plan;
+  FAV_REQUIRE(b >= 0 && b < pl->B, "fav_net_layer_output: image %d of a batch of %d", b, pl->B);
   auto it = pl->layer_operand.find(index);
   FAV_REQUIRE(it != pl->layer_operand.end(), "fav_net_layer_output: layer %d has no stored activation", index);
   const Operand &o = pl->ops[it->second];
@@ -878,11 +916,16 @@ int fav_net_layer_output(fav_net_t *net, int index, float *out, int *C, int *Hl,
   if (Hl) *Hl = o.H;
   if (Wl) *Wl = o.W;
   if (!out) return FAV_OK;
-  return launch_unpack_operand(o, out, (cudaStream_t)stream);
+  return launch_unpack_operand(image_of(o, b), out, (cudaStream_t)stream);
 }
 
 int fav_run_image(fav_net_t *net, const float *content, const float *fill, int H, int W, float *out_rgb,
                   void *stream) {
+  return fav_run_image_batch(net, content, fill, 1, H, W, out_rgb, stream);
+}
+
+int fav_run_image_batch(fav_net_t *net, const float *content, const float *fill, int B, int H, int W, float *out_rgb,
+                        void *stream) {
   FAV_REQUIRE(net && content && out_rgb, "fav_run_image: null argument");
   FAV_REQUIRE(net->finalized, "fav_run_image: call fav_net_finalize first");
   // model_img == nil: the video model on cat(pre(img), fill, zeros) (core.lua:133-138); a separate 3-channel image model
@@ -890,34 +933,41 @@ int fav_run_image(fav_net_t *net, const float *content, const float *fill, int H
   FAV_REQUIRE(net->in_dim == 7 || net->in_dim == 3, "fav_run_image: video model (7 input channels) or image model (3) required");
   if (net->in_dim == 3) fill = nullptr;
   Plan *pl;
-  FAV_TRY(build_plan(net, H, W, &pl));
+  FAV_TRY(build_plan(net, B, H, W, &pl));
   cudaStream_t st = (cudaStream_t)stream;
   static const bool fuse_pack = getenv("FAV_NO_FUSEPACK") == nullptr;
   if (fuse_pack) {
-    FAV_TRY(launch_temporal_input_packed(content, nullptr, nullptr, nullptr, fill, nullptr, pl->ops[0], net->reflect_pad, H, W, 0, true, st));
+    FAV_TRY(launch_temporal_input_packed(content, nullptr, nullptr, nullptr, fill, nullptr, pl->ops[0], net->reflect_pad, H, W, 0, true, st,
+                                         B));
     return run_plan_frame(net, *pl, nullptr, out_rgb, st);
   }
-  FAV_TRY(launch_temporal_input(content, nullptr, nullptr, nullptr, fill, nullptr, pl->in7, H, W, 0, true, st));
+  FAV_TRY(launch_temporal_input(content, nullptr, nullptr, nullptr, fill, nullptr, pl->in7, H, W, 0, true, st, B));
   return run_plan_frame(net, *pl, pl->in7, out_rgb, st);  // deprocess fused into the last epilogue (core.lua:149)
 }
 
 int fav_run_next_image(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow,
                        const float *cert, const float *fill, const float *flow_mask, int H, int W, int border_mode,
                        float *out_rgb, void *stream) {
+  return fav_run_next_image_batch(net, content, prev_rgb, flow, cert, fill, flow_mask, 1, H, W, border_mode, out_rgb, stream);
+}
+
+int fav_run_next_image_batch(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow,
+                             const float *cert, const float *fill, const float *flow_mask, int B, int H, int W, int border_mode,
+                             float *out_rgb, void *stream) {
   FAV_REQUIRE(net && content && prev_rgb && flow && cert && out_rgb, "fav_run_next_image: null argument");
   FAV_REQUIRE(net->finalized, "fav_run_next_image: call fav_net_finalize first");
   FAV_REQUIRE(net->in_dim == 7, "fav_run_next_image: video model (7 input channels) required");
   FAV_REQUIRE(border_mode == FAV_BORDER_PER_TAP || border_mode == FAV_BORDER_PAD_PIXEL, "bad border_mode");
   Plan *pl;
-  FAV_TRY(build_plan(net, H, W, &pl));
+  FAV_TRY(build_plan(net, B, H, W, &pl));
   cudaStream_t st = (cudaStream_t)stream;
   static const bool fuse_pack = getenv("FAV_NO_FUSEPACK") == nullptr;
   if (fuse_pack) {
     FAV_TRY(launch_temporal_input_packed(content, prev_rgb, flow, cert, fill, flow_mask, pl->ops[0], net->reflect_pad, H, W,
-                                         border_mode, false, st));
+                                         border_mode, false, st, B));
     return run_plan_frame(net, *pl, nullptr, out_rgb, st);
   }
-  FAV_TRY(launch_temporal_input(content, prev_rgb, flow, cert, fill, flow_mask, pl->in7, H, W, border_mode, false, st));
+  FAV_TRY(launch_temporal_input(content, prev_rgb, flow, cert, fill, flow_mask, pl->in7, H, W, border_mode, false, st, B));
   return run_plan_frame(net, *pl, pl->in7, out_rgb, st);  // core.lua:172-173
 }
 
@@ -926,6 +976,13 @@ int fav_run_next_image(fav_net_t *net, const float *content, const float *prev_r
 int fav_run_next_image_flows(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow_bw,
                              const float *flow_fw_uv, const float *cert_raw, const float *fill, const float *flow_mask,
                              int H, int W, int min_filter_r, int border_mode, float *out_rgb, void *stream) {
+  return fav_run_next_image_flows_batch(net, content, prev_rgb, flow_bw, flow_fw_uv, cert_raw, fill, flow_mask, 1, H, W,
+                                        min_filter_r, border_mode, out_rgb, stream);
+}
+
+int fav_run_next_image_flows_batch(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow_bw,
+                                   const float *flow_fw_uv, const float *cert_raw, const float *fill, const float *flow_mask,
+                                   int B, int H, int W, int min_filter_r, int border_mode, float *out_rgb, void *stream) {
   FAV_REQUIRE(net && content && prev_rgb && flow_bw && out_rgb, "fav_run_next_image_flows: null argument");
   FAV_REQUIRE((flow_fw_uv != nullptr) != (cert_raw != nullptr), "fav_run_next_image_flows: give either the forward flow or a certainty plane");
   FAV_REQUIRE(net->finalized, "fav_run_next_image_flows: call fav_net_finalize first");
@@ -933,29 +990,32 @@ int fav_run_next_image_flows(fav_net_t *net, const float *content, const float *
   FAV_REQUIRE(border_mode == FAV_BORDER_PER_TAP || border_mode == FAV_BORDER_PAD_PIXEL, "bad border_mode");
   FAV_REQUIRE(min_filter_r >= 0 && (min_filter_r <= 1 || (min_filter_r & 1)) && min_filter_r <= 15, "occlusions_min_filter must be odd <= 15");
   Plan *pl;
-  FAV_TRY(build_plan(net, H, W, &pl));
+  FAV_TRY(build_plan(net, B, H, W, &pl));
   cudaStream_t st = (cudaStream_t)stream;
   static const bool no_stage = getenv("FAV_NO_STAGE") != nullptr;  // A/B timing: the three separate kernels
   int rc = no_stage ? FAV_ERR_UNSUPPORTED
                     : launch_temporal_stage(content, prev_rgb, flow_bw, flow_fw_uv, cert_raw, fill, flow_mask, nullptr, nullptr,
-                                            &pl->ops[0], net->reflect_pad, H, W, min_filter_r, border_mode, st);
+                                            &pl->ops[0], net->reflect_pad, H, W, min_filter_r, border_mode, st, B);
   if (rc == FAV_ERR_UNSUPPORTED) {  // unaligned planes / W % 4 != 0: the three separate kernels
     const int64_t HW = (int64_t)H * W;
     if (!pl->cert_a) {
-      FAV_TRY(alloc_zero(*pl, (void **)&pl->cert_a, HW * sizeof(float)));
-      FAV_TRY(alloc_zero(*pl, (void **)&pl->cert_b, HW * sizeof(float)));
+      FAV_TRY(alloc_zero(*pl, (void **)&pl->cert_a, B * HW * sizeof(float)));
+      FAV_TRY(alloc_zero(*pl, (void **)&pl->cert_b, B * HW * sizeof(float)));
     }
     const float *cert = cert_raw;
     if (flow_fw_uv) {
-      FAV_TRY(launch_consistency(flow_bw + HW, flow_bw, flow_fw_uv, flow_fw_uv + HW, nullptr, nullptr, 0.f, nullptr, pl->cert_a, W, H, st));
+      for (int b = 0; b < B; ++b) {
+        const float *bw = flow_bw + 2 * b * HW, *fw = flow_fw_uv + 2 * b * HW;
+        FAV_TRY(launch_consistency(bw + HW, bw, fw, fw + HW, nullptr, nullptr, 0.f, nullptr, pl->cert_a + b * HW, W, H, st));
+      }
       cert = pl->cert_a;
     }
     if (min_filter_r > 1) {
-      FAV_TRY(launch_min_filter(cert, pl->cert_b, 1, H, W, min_filter_r, st));
+      FAV_TRY(launch_min_filter(cert, pl->cert_b, B, H, W, min_filter_r, st));
       cert = pl->cert_b;
     }
     rc = launch_temporal_input_packed(content, prev_rgb, flow_bw, cert, fill, flow_mask, pl->ops[0], net->reflect_pad, H, W,
-                                      border_mode, false, st);
+                                      border_mode, false, st, B);
   }
   FAV_TRY(rc);
   return run_plan_frame(net, *pl, nullptr, out_rgb, st);

@@ -10,6 +10,7 @@
 namespace fav {
 
 constexpr int kStatRows = 8;
+
 constexpr int kApplyIter = 4;  // pixels per thread in the apply kernels: amortises the per-block finalisation
 
 __device__ __forceinline__ void load_join8(const uint4 *hi_src, const uint4 *lo_src, float v[8]) {
@@ -27,12 +28,15 @@ __device__ __forceinline__ void load_join8(const uint4 *hi_src, const uint4 *lo_
 // ---- pack_input --------------------------------------------------------------------------------------
 // in: [Cin][H][W] fp32.  dst logical size = (H+2R) x (W+2R) with R = reflect (nn.SpatialReflectionPadding:
 // index -i for i<0, 2(n-1)-i for i>=n).  One thread per (padded pixel, channel block).
+// Batch: blockIdx.z = b * Cb + cb, in [nimg][Cin][H][W].
 __global__ void __launch_bounds__(256) pack_input_kernel(const float *__restrict__ in, int Cin, int H, int W, int R,
                                                          Operand dst) {
   int x = blockIdx.x * blockDim.x + threadIdx.x;
   int y = blockIdx.y;
-  int cb = blockIdx.z;
+  const int b = blockIdx.z / dst.Cb, cb = blockIdx.z - b * dst.Cb;
   if (x >= dst.W) return;
+  in += (int64_t)b * Cin * H * W;
+  dst = image_of(dst, b);
   int sy = y - R, sx = x - R;
   sy = sy < 0 ? -sy : (sy >= H ? 2 * (H - 1) - sy : sy);
   sx = sx < 0 ? -sx : (sx >= W ? 2 * (W - 1) - sx : sx);
@@ -46,15 +50,18 @@ __global__ void __launch_bounds__(256) pack_input_kernel(const float *__restrict
   split_store8(v, reinterpret_cast<uint4 *>(dst.hi) + o, reinterpret_cast<uint4 *>(dst.lo) + o);
 }
 
-int launch_pack_input(const float *in, int Cin, int H, int W, int reflect, const Operand &dst, cudaStream_t st) {
-  dim3 grid(ceil_div(dst.W, 256), dst.H, dst.Cb);
+int launch_pack_input(const float *in, int Cin, int H, int W, int reflect, const Operand &dst, cudaStream_t st, int nimg) {
+  dim3 grid(ceil_div(dst.W, 256), dst.H, dst.Cb * nimg);
   pack_input_kernel<<<grid, 256, 0, st>>>(in, Cin, H, W, reflect, dst);
   return post_launch("pack_input");
 }
 
 // ---- in_stats ----------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) in_stats_kernel(RawTensor raw, double *__restrict__ sums) {
+// Batch: blockIdx.z = image
+__global__ void __launch_bounds__(256) in_stats_kernel(RawTensor raw, double *__restrict__ sums, int64_t sums_img) {
   const int cq = blockIdx.x;
+  raw = image_of(raw, blockIdx.z);
+  sums += blockIdx.z * sums_img;
   const int y0 = blockIdx.y * kStatRows;
   float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
   for (int y = y0; y < min(y0 + kStatRows, raw.H); ++y) {
@@ -94,23 +101,27 @@ __global__ void __launch_bounds__(256) in_stats_kernel(RawTensor raw, double *__
   }
 }
 
-int launch_in_stats(const RawTensor &raw, double *sums, cudaStream_t st) {
-  dim3 grid(raw.Cq, ceil_div(raw.H, kStatRows));
-  in_stats_kernel<<<grid, 256, 0, st>>>(raw, sums);
+int launch_in_stats(const RawTensor &raw, double *sums, cudaStream_t st, int nimg, int64_t sums_img) {
+  dim3 grid(raw.Cq, ceil_div(raw.H, kStatRows), nimg);
+  in_stats_kernel<<<grid, 256, 0, st>>>(raw, sums, sums_img);
   return post_launch("in_stats");
 }
 
 // ---- in_apply ----------------------------------------------------------------------------------------
 // mean / gamma*rstd / beta of the block's 8 channels are derived from the (double) sums by the first 8 threads:
-// biased variance, eps inside the sqrt (nn.SpatialBatchNormalization in training mode, InstanceNormalization.lua:39-50)
+// biased variance, eps inside the sqrt (nn.SpatialBatchNormalization in training mode, InstanceNormalization.lua:39-50).
+// Batch: blockIdx.z = b * (C / 8) + cb, statistics of image b at sums + b * sums_img.
 template <int ITER>
 __global__ void __launch_bounds__(128) in_apply_kernel(RawTensor raw, const double *__restrict__ sums,
                                                        const float *__restrict__ gamma, const float *__restrict__ beta,
                                                        double inv_count, double eps, int relu, Operand skip, int has_skip,
-                                                       int shave, Operand dst) {
+                                                       int shave, Operand dst, int64_t sums_img) {
   __shared__ float s_mean[8], s_scale[8], s_beta[8];
   const int xbase = blockIdx.x * (128 * ITER) + threadIdx.x;
-  const int y = blockIdx.y, cb = blockIdx.z;
+  const int y = blockIdx.y, b = blockIdx.z / (raw.C / 8), cb = blockIdx.z - b * (raw.C / 8);
+  raw = image_of(raw, b); dst = image_of(dst, b);
+  if (has_skip) skip = image_of(skip, b);
+  if (sums) sums += b * sums_img;
   // 1. every streaming load of the thread is requested first (they do not depend on the statistics): the per-block
   //    finalisation below (dependent global loads + double sqrt / divide on 8 threads) then runs in their shadow
   float v[ITER][8];
@@ -173,19 +184,19 @@ __global__ void __launch_bounds__(128) in_apply_kernel(RawTensor raw, const doub
 }
 
 int launch_in_apply(const RawTensor &raw, const double *sums, const float *gamma, const float *beta, float eps, int relu,
-                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st) {
+                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st, int nimg, int64_t sums_img) {
   // pixels per thread: amortises the per-block finalisation against registers (occupancy); FAV_APPLY_ITER = 2|3|4 for A/B timing
   static const int forced = getenv("FAV_APPLY_ITER") ? atoi(getenv("FAV_APPLY_ITER")) : 0;
   const int iter = forced >= 2 && forced <= 4 ? forced : kApplyIter;
-  dim3 grid(ceil_div(raw.W, 128 * iter), raw.H, raw.C / 8);
+  dim3 grid(ceil_div(raw.W, 128 * iter), raw.H, raw.C / 8 * nimg);
   Operand sk = skip ? *skip : Operand();
   const double inv = 1.0 / ((double)raw.H * raw.W);
   if (iter == 2)
-    in_apply_kernel<2><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst);
+    in_apply_kernel<2><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img);
   else if (iter == 3)
-    in_apply_kernel<3><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst);
+    in_apply_kernel<3><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img);
   else
-    in_apply_kernel<4><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst);
+    in_apply_kernel<4><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img);
   return post_launch("in_apply");
 }
 
@@ -198,8 +209,11 @@ int launch_in_apply(const RawTensor &raw, const double *sums, const float *gamma
 // ---- nn.SpatialUpSamplingNearest(s) -> InstanceNormalization -> ReLU on an OPERAND (arch token UX) ---------------
 // models_video.lua:94-98,121-130.  Statistics of a nearest-upsampled tensor equal those of its source, so the sums
 // are taken over the source operand and the upsampling happens while the normalised values are written.
-__global__ void __launch_bounds__(256) opnd_stats_kernel(Operand src, double *__restrict__ sums) {
+// Batch: blockIdx.z = image
+__global__ void __launch_bounds__(256) opnd_stats_kernel(Operand src, double *__restrict__ sums, int64_t sums_img) {
   const int cb = blockIdx.x;
+  src = image_of(src, blockIdx.z);
+  sums += blockIdx.z * sums_img;
   const int y0 = blockIdx.y * kStatRows;
   float s[8], q[8];
 #pragma unroll
@@ -236,10 +250,13 @@ __global__ void __launch_bounds__(256) opnd_stats_kernel(Operand src, double *__
 __global__ void __launch_bounds__(128) up_apply_kernel(Operand src, const double *__restrict__ sums,
                                                        const float *__restrict__ gamma, const float *__restrict__ beta,
                                                        double inv_count, double eps, int relu, int scale, Operand dst,
-                                                       const float *__restrict__ tab_mean, const float *__restrict__ tab_scale) {
+                                                       const float *__restrict__ tab_mean, const float *__restrict__ tab_scale,
+                                                       int64_t sums_img) {
   __shared__ float s_mean[8], s_scale[8], s_beta[8];
   const int xbase = blockIdx.x * (128 * kApplyIter) + threadIdx.x;
-  const int y = blockIdx.y, cb = blockIdx.z;
+  const int y = blockIdx.y, b = blockIdx.z / dst.Cb, cb = blockIdx.z - b * dst.Cb;  // batch: blockIdx.z = b * Cb + cb
+  src = image_of(src, b); dst = image_of(dst, b);
+  if (sums) sums += b * sums_img;
   if (threadIdx.x < 8) {
     int c = cb * 8 + threadIdx.x;
     if (tab_scale) {  // inference-mode BatchNorm after the upsampling: running mean, weight / sqrt(running_var + eps)
@@ -268,14 +285,14 @@ __global__ void __launch_bounds__(128) up_apply_kernel(Operand src, const double
 }
 
 int launch_up_in(const Operand &src, double *sums, const float *gamma, const float *beta, float eps, int relu, int scale,
-                 const Operand &dst, cudaStream_t st, const float *tab_mean, const float *tab_scale) {
+                 const Operand &dst, cudaStream_t st, const float *tab_mean, const float *tab_scale, int nimg, int64_t sums_img) {
   if (!tab_scale) {
-    opnd_stats_kernel<<<dim3(src.Cb, ceil_div(src.H, kStatRows)), 256, 0, st>>>(src, sums);
+    opnd_stats_kernel<<<dim3(src.Cb, ceil_div(src.H, kStatRows), nimg), 256, 0, st>>>(src, sums, sums_img);
     FAV_TRY(post_launch("up_in.stats"));
   }
-  dim3 grid(ceil_div(dst.W, 128 * kApplyIter), dst.H, dst.Cb);
+  dim3 grid(ceil_div(dst.W, 128 * kApplyIter), dst.H, dst.Cb * nimg);
   up_apply_kernel<<<grid, 128, 0, st>>>(src, sums, gamma, beta, 1.0 / ((double)src.H * src.W), (double)eps, relu, scale, dst,
-                                        tab_mean, tab_scale);
+                                        tab_mean, tab_scale, sums_img);
   return post_launch("up_in.apply");
 }
 

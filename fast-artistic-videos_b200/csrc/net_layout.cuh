@@ -31,6 +31,7 @@ struct Operand {
   int Hs = 0, Ws = 0;       // storage rows / pixels per (row, cb) slab (non-parity)
   int parity = 0, Ws2 = 0;  // parity split: slab = [2][Ws2]
   size_t elems16 = 0;       // allocation size in 16-byte units (per hi / lo), incl. tail slack
+  int64_t img16 = 0;        // a batch of images: image b's hi / lo planes start b * img16 16-byte units in (own zero border)
   __host__ __device__ int slab16() const { return parity ? 2 * Ws2 : Ws; }
   // offset in 16-byte units of storage pixel (ys, xs) of channel block cb
   __host__ __device__ int64_t off16(int ys, int cb, int xs) const {
@@ -82,9 +83,20 @@ struct RawTensor {
   int H = 0, W = 0;   // logical size
   int Hp = 0, Wp = 0; // allocated rows / row pitch in pixels (multiple of 128; planar: multiple of 16)
   int planar = 0;     // 1: fp32 [C][Hp][Wp]; 0: [Ho][Cq][Wp][4]
+  int64_t img = 0;    // a batch of images: image b's tensor starts b * img floats in
   __host__ __device__ int64_t off4(int y, int cq, int x) const { return (((int64_t)y * Cq + cq) * Wp + x); }
   __host__ __device__ int64_t offp(int c, int y, int x) const { return (((int64_t)c * Hp + y) * Wp + x); }
 };
+
+// image b of a batch (Operand::img16, RawTensor::img): the same tensor with its pointers moved to that image
+__host__ __device__ inline Operand image_of(Operand o, int b) {
+  o.hi += b * o.img16 * 8; o.lo += b * o.img16 * 8;
+  return o;
+}
+__host__ __device__ inline RawTensor image_of(RawTensor r, int b) {
+  r.p += b * r.img;
+  return r;
+}
 
 // one filter tap of a (phase of a) convolution: input pixel = (sy*y + dy, sx*x + dx)
 struct ConvTap {

@@ -100,6 +100,13 @@ SIGNATURES = {
     "fav_run_image": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, _fp, _fp]),
     "fav_run_next_image": (C.c_int, [C.c_void_p, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]),
     "fav_run_next_image_flows": (C.c_int, [C.c_void_p, _fp, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp, _fp]),
+    "fav_net_forward_batch": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]),
+    "fav_net_layer_output_image": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                             C.POINTER(C.c_int), _fp]),
+    "fav_run_image_batch": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]),
+    "fav_run_next_image_batch": (C.c_int, [C.c_void_p, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp, _fp]),
+    "fav_run_next_image_flows_batch": (C.c_int, [C.c_void_p, _fp, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                 C.c_int, _fp, _fp]),
     "fav_session_create": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "fav_session_destroy": (None, [C.c_void_p]),
     "fav_session_set_image_model": (C.c_int, [C.c_void_p, C.c_void_p]),

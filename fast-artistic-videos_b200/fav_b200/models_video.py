@@ -1,7 +1,11 @@
 """fast_artistic_video/models_video.lua -- `models_video.build_model(opt)` (:55-140).
 
-Returns a StyleNet whose `forward(input[1x7xHxW]) -> [1x3xHxW]` runs the sm_90a path
-(fav_net_forward, include/fav.h).  Parameters are addressed by the names listed in fav.h.
+Returns a StyleNet whose `forward(input[Nx7xHxW]) -> [Nx3xHxW]` runs the sm_90a path
+(fav_net_forward_batch, include/fav.h).  Parameters are addressed by the names listed in fav.h.
+
+Batches: like the reference nn modules, forward takes N >= 1 images of one size, and run_image / run_next_image /
+run_next_image_flows accept a leading batch dimension.  A batch runs through one plan in one launch per kernel; image b of
+the result is bit-identical to that image run alone.
 """
 from __future__ import annotations
 
@@ -65,13 +69,13 @@ class StyleNet:
 
     # -- model:forward(input) ----------------------------------------------------------------------
     def forward(self, input: torch.Tensor) -> torch.Tensor:
-        assert input.dim() == 4 and input.size(0) == 1 and input.size(1) == self.in_dim, \
-            f"expected 1x{self.in_dim}xHxW input"
+        assert input.dim() == 4 and input.size(0) >= 1 and input.size(1) == self.in_dim, \
+            f"expected Nx{self.in_dim}xHxW input"
         x = input.contiguous()
         assert x.dtype == torch.float32
-        H, W = x.shape[-2:]
-        out = torch.empty((1, 3, H, W), dtype=torch.float32, device=x.device)
-        _lib.check(_lib.lib.fav_net_forward(self._h, _lib.dptr(x), H, W, _lib.dptr(out), _lib.stream_ptr()))
+        N, (H, W) = x.size(0), x.shape[-2:]
+        out = torch.empty((N, 3, H, W), dtype=torch.float32, device=x.device)
+        _lib.check(_lib.lib.fav_net_forward_batch(self._h, _lib.dptr(x), N, H, W, _lib.dptr(out), _lib.stream_ptr()))
         return out
 
     def profile(self, input: torch.Tensor):
@@ -89,48 +93,91 @@ class StyleNet:
         return [dict(kind=kn[kinds[i]], name=names.raw[24 * i:24 * i + 24].split(b"\0")[0].decode(), ms=float(ms[i]),
                      work=float(work[i])) for i in range(n.value)]
 
-    def layer_output(self, index: int) -> torch.Tensor:
+    def layer_output(self, index: int, image: int = 0) -> torch.Tensor:
+        """Activation after layer `index` of image `image` of the last forward's batch."""
         c, h, w = C.c_int(), C.c_int(), C.c_int()
-        _lib.check(_lib.lib.fav_net_layer_output(self._h, index, None, C.byref(c), C.byref(h), C.byref(w), None))
+        _lib.check(_lib.lib.fav_net_layer_output_image(self._h, index, image, None, C.byref(c), C.byref(h), C.byref(w), None))
         out = torch.empty((c.value, h.value, w.value), dtype=torch.float32, device="cuda")
-        _lib.check(_lib.lib.fav_net_layer_output(self._h, index, _lib.dptr(out), C.byref(c), C.byref(h), C.byref(w),
-                                                 _lib.stream_ptr()))
+        _lib.check(_lib.lib.fav_net_layer_output_image(self._h, index, image, _lib.dptr(out), C.byref(c), C.byref(h),
+                                                       C.byref(w), _lib.stream_ptr()))
         return out
 
     # -- fused frame-level ops (fast_artistic_video_core.lua:121-180) ------------------------------------
     def run_image(self, img: torch.Tensor, fill: torch.Tensor = None) -> torch.Tensor:
+        """img [3,H,W], or [B,3,H,W] for a batch (fill then [B,3,H,W] too)."""
         x = img.contiguous()
-        assert x.dim() == 3 and x.size(0) == 3 and x.dtype == torch.float32
+        assert x.dim() in (3, 4) and x.size(-3) == 3 and x.dtype == torch.float32
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
-        _lib.check(_lib.lib.fav_run_image(self._h, _lib.dptr(x), _lib.dptr(fill), H, W, _lib.dptr(out),
-                                          _lib.stream_ptr()))
+        if x.dim() == 3:
+            _lib.check(_lib.lib.fav_run_image(self._h, _lib.dptr(x), _lib.dptr(fill), H, W, _lib.dptr(out),
+                                              _lib.stream_ptr()))
+        else:
+            fill = _planes(fill, x, 3)
+            _lib.check(_lib.lib.fav_run_image_batch(self._h, _lib.dptr(x), _lib.dptr(fill), x.size(0), H, W, _lib.dptr(out),
+                                                    _lib.stream_ptr()))
         return out
 
     def run_next_image(self, img, prev_rgb, flow, cert, fill=None, flow_mask=None,
                        border_mode=_lib.BORDER_PER_TAP) -> torch.Tensor:
-        x, p, f, c = img.contiguous(), prev_rgb.contiguous(), flow.contiguous(), cert.contiguous()
+        """img / prev_rgb [3,H,W], flow [2,H,W], cert [H,W]; or all of them (and fill, flow_mask) with a leading batch
+        dimension B: B independent clips advance one frame, each from its own prev_rgb[b]."""
+        x = img.contiguous()
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
-        _lib.check(_lib.lib.fav_run_next_image(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(c),
-                                               _lib.dptr(fill), _lib.dptr(flow_mask), H, W, border_mode,
-                                               _lib.dptr(out), _lib.stream_ptr()))
+        if x.dim() == 3:
+            p, f, c = prev_rgb.contiguous(), flow.contiguous(), cert.contiguous()
+            _lib.check(_lib.lib.fav_run_next_image(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(c),
+                                                   _lib.dptr(fill), _lib.dptr(flow_mask), H, W, border_mode,
+                                                   _lib.dptr(out), _lib.stream_ptr()))
+        else:
+            p, f, c = _planes(prev_rgb, x, 3), _planes(flow, x, 2), _planes(cert, x, 0)
+            fill, flow_mask = _planes(fill, x, 3), _planes(flow_mask, x, 0)
+            _lib.check(_lib.lib.fav_run_next_image_batch(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(c),
+                                                         _lib.dptr(fill), _lib.dptr(flow_mask), x.size(0), H, W, border_mode,
+                                                         _lib.dptr(out), _lib.stream_ptr()))
         return out
 
 
     def run_next_image_flows(self, img, prev_rgb, flow_bw, flow_fw_uv=None, cert_raw=None, min_filter_r=7, fill=None,
                              flow_mask=None, border_mode=_lib.BORDER_PER_TAP) -> torch.Tensor:
         """run_next_image with func_load_cert + utils.min_filter inside (fav_run_next_image_flows): the whole temporal stage is
-        ONE kernel.  flow_bw [2,H,W] (dy,dx); flow_fw_uv [2,H,W] (u,v) -> occlusion test on the GPU, or cert_raw [H,W]."""
-        x, p, f = img.contiguous(), prev_rgb.contiguous(), flow_bw.contiguous()
-        fw = None if flow_fw_uv is None else flow_fw_uv.contiguous()
-        cr = None if cert_raw is None else cert_raw.contiguous()
+        ONE kernel.  flow_bw [2,H,W] (dy,dx); flow_fw_uv [2,H,W] (u,v) -> occlusion test on the GPU, or cert_raw [H,W].
+        A leading batch dimension B on every argument: B independent clips advance one frame."""
+        x = img.contiguous()
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
-        _lib.check(_lib.lib.fav_run_next_image_flows(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(fw), _lib.dptr(cr),
-                                                     _lib.dptr(fill), _lib.dptr(flow_mask), H, W, int(min_filter_r), border_mode,
-                                                     _lib.dptr(out), _lib.stream_ptr()))
+        if x.dim() == 3:
+            p, f = prev_rgb.contiguous(), flow_bw.contiguous()
+            fw = None if flow_fw_uv is None else flow_fw_uv.contiguous()
+            cr = None if cert_raw is None else cert_raw.contiguous()
+            _lib.check(_lib.lib.fav_run_next_image_flows(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(fw),
+                                                         _lib.dptr(cr), _lib.dptr(fill), _lib.dptr(flow_mask), H, W,
+                                                         int(min_filter_r), border_mode, _lib.dptr(out), _lib.stream_ptr()))
+        else:
+            p, f = _planes(prev_rgb, x, 3), _planes(flow_bw, x, 2)
+            fw, cr = _planes(flow_fw_uv, x, 2), _planes(cert_raw, x, 0)
+            fill, flow_mask = _planes(fill, x, 3), _planes(flow_mask, x, 0)
+            _lib.check(_lib.lib.fav_run_next_image_flows_batch(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(fw),
+                                                               _lib.dptr(cr), _lib.dptr(fill), _lib.dptr(flow_mask), x.size(0), H,
+                                                               W, int(min_filter_r), border_mode, _lib.dptr(out),
+                                                               _lib.stream_ptr()))
         return out
+
+
+def _planes(t, img, c):
+    """t (or None) as a contiguous tensor of `c` planes per image of the batch img [B,3,H,W]; c = 0: one plane without a
+    channel dimension ([B,H,W]; [B,1,H,W] is accepted as well).  Mismatched shapes raise
+    FavError(FAV_ERR_INVALID) before anything is launched."""
+    if t is None:
+        return None
+    lead, (H, W) = tuple(img.shape[:-3]), tuple(img.shape[-2:])
+    want = lead + ((c,) if c else ()) + (H, W)
+    if c == 0 and t.dim() == len(want) + 1 and t.size(-3) == 1:
+        t = t.reshape(want)
+    if tuple(t.shape) != want or t.dtype != torch.float32:
+        raise _lib.FavError(_lib.FAV_ERR_INVALID, f"expected a float32 tensor of shape {list(want)}, got {t.dtype} {list(t.shape)}")
+    return t.contiguous()
 
 
 def build_model(opt) -> StyleNet:

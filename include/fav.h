@@ -213,6 +213,18 @@ FAV_API int fav_net_profile(fav_net_t *net, const float *in7, int H, int W, floa
 FAV_API int fav_net_layer_output(fav_net_t *net, int index, float *out, int *C, int *Hl, int *Wl,
                                  void *stream);
 
+/* Batches.  The reference nets are nn modules that take N x C x H x W (InstanceNormalization.lua:33-53 normalises per (n, c);
+ * train_video.lua:60 trains with -batch_size 4).  The *_batch calls take B frames of one size stored one after the other and run
+ * them through one plan: every kernel covers all B images in one launch, and a run_* call is still ONE graph launch.  Image b of
+ * a batch is bit-identical to the same frame run alone.  B = 1 is the single-frame call.  FAV_ERR_INVALID for B < 1, B > 64, or
+ * a batch whose activation buffers would exceed 32 GiB (checked before they are allocated).
+ *
+ * model:forward(input) of a batch                fast_artistic_video_core.lua:138,172
+ * in [B,in_dim,H,W] device fp32 -> out3 [B,3,H,W] device fp32 in net space. */
+FAV_API int fav_net_forward_batch(fav_net_t *net, const float *in, int B, int H, int W, float *out3, void *stream);
+/* fav_net_layer_output for image b of the last forward's batch (models_video.lua:55-140 layer `index`). */
+FAV_API int fav_net_layer_output_image(fav_net_t *net, int index, int b, float *out, int *C, int *Hl, int *Wl, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * f-5  the perceptual loss network of -evaluate: nn.PerceptualCriterion with nn.ContentLoss / nn.StyleLoss
  *      (fast_artistic_video/PerceptualCriterion.lua:27-155, ContentLoss.lua:39-48, StyleLoss.lua:39-55,
@@ -281,6 +293,22 @@ FAV_API int fav_run_next_image_flows(fav_net_t *net, const float *content, const
                                      const float *flow_fw_uv, const float *cert_raw, const float *fill,
                                      const float *flow_mask, int H, int W, int min_filter_r, int border_mode,
                                      float *out_rgb, void *stream);
+
+/* Batched frame calls (see fav_net_forward_batch): every plane argument holds B images one after the other -- content,
+ * prev_rgb, fill, out_rgb [B,3,H,W]; flow, flow_bw, flow_fw_uv [B,2,H,W]; cert, cert_raw, flow_mask [B,H,W].  Each image keeps
+ * its own recurrent state (the caller's prev_rgb[b]), so B independent clips advance one frame per call.
+ *   run_image                                    fast_artistic_video_core.lua:121-158 */
+FAV_API int fav_run_image_batch(fav_net_t *net, const float *content, const float *fill, int B, int H, int W, float *out_rgb,
+                                void *stream);
+/*   run_next_image                               fast_artistic_video_core.lua:161-180 */
+FAV_API int fav_run_next_image_batch(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow,
+                                     const float *cert, const float *fill, const float *flow_mask, int B, int H, int W,
+                                     int border_mode, float *out_rgb, void *stream);
+/*   run_next_image with func_load_cert + utils.min_filter inside (core.lua:206-208) */
+FAV_API int fav_run_next_image_flows_batch(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow_bw,
+                                           const float *flow_fw_uv, const float *cert_raw, const float *fill,
+                                           const float *flow_mask, int B, int H, int W, int min_filter_r, int border_mode,
+                                           float *out_rgb, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a-10  frame loop with HOST buffers (the reference-facing call bench.py's e2e times)
