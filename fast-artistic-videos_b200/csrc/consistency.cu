@@ -11,6 +11,7 @@
 // The motion-edge branch (:129-132) assigns MOTION_BOUNDARIE_VALUE = 255 (:12) to pixels that are
 // already 255 and is therefore not evaluated (no observable effect).
 #include "fav_common.cuh"
+#include "exact_avg.cuh"
 #include "occlusion.cuh"
 
 namespace fav {
@@ -66,8 +67,8 @@ int launch_consistency(const float *f1u, const float *f1v, const float *f2u, con
 //      for dxx, dyy, dxy -- the recurrences are sequential per line, as in the reference
 //   3. smallest eigenvalue (parallel)
 //   4. normalize(0,1): the reference's `else if` min/max scan is evaluated EXACTLY by a parallel prefix-maximum scan
-//      (norm_*_kernel); the fp32 avg is order-dependent by rounding and stays one sequential FADD chain fed through
-//      shared memory by the rest of the block (avg_scan_kernel).
+//      (norm_*_kernel); the fp32 avg, order-dependent by rounding, EXACTLY by integer runs within a binade (exact_avg.cuh,
+//      avg_*_kernel).
 // ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float deriv3(float m1, float c0, float p1) {
   // sum over i=-1,0,1 of f[i]*v starting from 0 (CFilter.h:1510-1514): ((0 + -0.5*m1) + 0*c0) + 0.5*p1
@@ -77,7 +78,9 @@ __device__ __forceinline__ float deriv3(float m1, float c0, float p1) {
   return s;
 }
 
-__global__ void __launch_bounds__(256) structure_tensor_kernel(const float *__restrict__ img, int Z, int W, int H,
+// scale: the image planes times `scale` are CTensor's 0..255 planes (1 for such planes; 255 for a frame of byte/255 values,
+// where fl(fl(byte/255) * 255) == byte for every byte)
+__global__ void __launch_bounds__(256) structure_tensor_kernel(const float *__restrict__ img, float scale, int Z, int W, int H,
                                                                float *__restrict__ dxx, float *__restrict__ dyy,
                                                                float *__restrict__ dxy) {
   int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
@@ -89,9 +92,9 @@ __global__ void __launch_bounds__(256) structure_tensor_kernel(const float *__re
   float sxx = 0.f, syy = 0.f, sxy = 0.f;
   for (int k = 0; k < Z; ++k) {  // consistencyChecker.cpp:55-61
     const float *p = img + k * n;
-    float c0 = __ldg(p + o);
-    float gx = deriv3(__ldg(p + (int64_t)y * W + xm), c0, __ldg(p + (int64_t)y * W + xp));
-    float gy = deriv3(__ldg(p + (int64_t)ym * W + x), c0, __ldg(p + (int64_t)yp * W + x));
+    float c0 = __fmul_rn(__ldg(p + o), scale);
+    float gx = deriv3(__fmul_rn(__ldg(p + (int64_t)y * W + xm), scale), c0, __fmul_rn(__ldg(p + (int64_t)y * W + xp), scale));
+    float gy = deriv3(__fmul_rn(__ldg(p + (int64_t)ym * W + x), scale), c0, __fmul_rn(__ldg(p + (int64_t)yp * W + x), scale));
     sxx = __fadd_rn(sxx, __fmul_rn(gx, gx));
     syy = __fadd_rn(syy, __fmul_rn(gy, gy));
     sxy = __fadd_rn(sxy, __fmul_rn(gx, gy));
@@ -289,44 +292,161 @@ __global__ void __launch_bounds__(256) normalize_apply_kernel(float *__restrict_
   m[i] = __fadd_rn(v, 0.0f);
 }
 // CMatrix::avg (CMatrix.h:1245-1251) adds the elements IN ORDER in fp32: every partial sum is rounded, so the result depends on
-// the order and no reassociated (parallel) sum reproduces it bit for bit.  It stays a sequential chain of dependent FADDs
-// (4 cycles each: ~2 ms per 720p frame, the floor of a single chain); what parallelises is everything around it: the block
-// streams the data through shared memory (double buffered, coalesced) so that the summing thread never waits for DRAM.
-constexpr int kAvgChunk = 4096;
-__global__ void __launch_bounds__(256) avg_scan_kernel(const float *__restrict__ m, int64_t n, float *__restrict__ avg) {
-  __shared__ __align__(16) float buf[2][kAvgChunk + 16];  // +16: the summing thread prefetches one batch past the chunk
-  const int64_t nchunks = (n + kAvgChunk - 1) / kAvgChunk;
-  auto load = [&](int64_t c, int s, int first, int stride) {  // the tail of the last chunk is +0.0f: a + 0 = a exactly
-    for (int i = first; i < kAvgChunk; i += stride) {
-      const int64_t g = c * kAvgChunk + i;
-      buf[s][i] = g < n ? m[g] : 0.f;
-    }
-  };
-  if (threadIdx.x < 32) buf[threadIdx.x >> 4][kAvgChunk + (threadIdx.x & 15)] = 0.f;
-  load(0, 0, threadIdx.x, 256);
-  __syncthreads();
-  float a = 0.f;
-  for (int64_t c = 0; c < nchunks; ++c) {
-    const int s = (int)(c & 1);
-    if (threadIdx.x == 0) {
-      // 16 values per batch, the next batch's four LDS.128 are in flight while this batch's 16 dependent FADDs retire
-      const float4 *b4 = reinterpret_cast<const float4 *>(buf[s]);
-      float4 r0 = b4[0], r1 = b4[1], r2 = b4[2], r3 = b4[3];
-      for (int i = 0; i < kAvgChunk / 16; ++i) {
-        const float4 n0 = b4[4 * i + 4], n1 = b4[4 * i + 5], n2 = b4[4 * i + 6], n3 = b4[4 * i + 7];
-        a = __fadd_rn(a, r0.x); a = __fadd_rn(a, r0.y); a = __fadd_rn(a, r0.z); a = __fadd_rn(a, r0.w);
-        a = __fadd_rn(a, r1.x); a = __fadd_rn(a, r1.y); a = __fadd_rn(a, r1.z); a = __fadd_rn(a, r1.w);
-        a = __fadd_rn(a, r2.x); a = __fadd_rn(a, r2.y); a = __fadd_rn(a, r2.z); a = __fadd_rn(a, r2.w);
-        a = __fadd_rn(a, r3.x); a = __fadd_rn(a, r3.y); a = __fadd_rn(a, r3.z); a = __fadd_rn(a, r3.w);
-        r0 = n0; r1 = n1; r2 = n2; r3 = n3;
-      }
-    } else if (c + 1 < nchunks) {
-      load(c + 1, s ^ 1, threadIdx.x - 1, 255);
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *avg = __fdiv_rn(a, (float)(int)n);
+// the order.  Evaluated exactly in parallel (exact_avg.cuh): double sums of the sub-chunks and chunks (the estimate that picks
+// the hypotheses) -> one block per chunk runs every (sub-chunk, hypothesis) in integers and composes the chunk's records -> one
+// warp combines the chunks in order from the exact state.
+struct AvgWs {
+  double *ssum, *csum;
+  AvgRec *srec, *crec;
+  int64_t nsub;
+  int nch;
+};
+__host__ __device__ inline size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+static size_t avg_ws_bytes(int64_t n) {
+  const int64_t nsub = ceil_div64(n, kAvgSub), nch = ceil_div64(nsub, kAvgGroup);
+  return align16(nsub * sizeof(double)) + align16(nch * sizeof(double)) + align16(nsub * sizeof(AvgRec)) +
+         align16(nch * sizeof(AvgRec)) + 16;
 }
+static AvgWs avg_ws(void *base, int64_t n) {
+  AvgWs w;
+  w.nsub = ceil_div64(n, kAvgSub);
+  w.nch = (int)ceil_div64(w.nsub, kAvgGroup);
+  char *p = (char *)(((uintptr_t)base + 15) & ~(uintptr_t)15);
+  w.ssum = (double *)p; p += align16(w.nsub * sizeof(double));
+  w.csum = (double *)p; p += align16(w.nch * sizeof(double));
+  w.srec = (AvgRec *)p; p += align16(w.nsub * sizeof(AvgRec));
+  w.crec = (AvgRec *)p;
+  return w;
+}
+
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// one block per chunk: the double sum of each sub-chunk and of the chunk
+__global__ void __launch_bounds__(256) avg_sum_kernel(const float *__restrict__ m, int64_t n, double *__restrict__ ssum,
+                                                      double *__restrict__ csum) {
+  __shared__ double part[8];
+  const int c = blockIdx.x, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t nsub = ceil_div64(n, kAvgSub);
+  double cs = 0.0;
+  for (int g = w; g < kAvgGroup; g += 8) {
+    const int64_t s = (int64_t)c * kAvgGroup + g;
+    if (s >= nsub) break;
+    double v = 0.0;
+    for (int i = lane; i < kAvgSub; i += 32) {
+      const int64_t e = s * kAvgSub + i;
+      if (e < n) v += (double)__ldg(m + e);
+    }
+    v = warp_sum_d(v);
+    if (lane == 0) ssum[s] = v;
+    cs += v;
+  }
+  if (lane == 0) part[w] = cs;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int k = 0; k < 8; ++k) t += part[k];
+    csum[c] = t;
+  }
+}
+
+// one block per chunk, one thread per (sub-chunk, hypothesis): the sub-chunks' records, then the chunk's records composed from them
+constexpr int kAvgHypThreads = kAvgGroup * kAvgHyps;
+__global__ void __launch_bounds__(kAvgHypThreads) avg_hyp_kernel(const float *__restrict__ m, int64_t n,
+                                                                 const double *__restrict__ ssum, const double *__restrict__ csum,
+                                                                 AvgRec *__restrict__ srec, AvgRec *__restrict__ crec) {
+  __shared__ double red[kAvgHypThreads / 32];
+  __shared__ int32_t seb[kAvgGroup];
+  __shared__ AvgHyp sh[kAvgGroup][kAvgHyps];
+  const int c = blockIdx.x, t = threadIdx.x;
+  const int64_t nsub = ceil_div64(n, kAvgSub), s0 = (int64_t)c * kAvgGroup;
+  const int ns = (int)min((int64_t)kAvgGroup, nsub - s0);
+  double p = 0.0;  // the estimate of the running sum before this chunk
+  for (int i = t; i < c; i += kAvgHypThreads) p += csum[i];
+  p = warp_sum_d(p);
+  if ((t & 31) == 0) red[t >> 5] = p;
+  __syncthreads();
+  if (t == 0) {
+    double S = 0.0;
+    for (int k = 0; k < kAvgHypThreads / 32; ++k) S += red[k];
+    const int32_t eb = avg_estimate_exp(S);
+    crec[c].ebase = eb;
+    for (int g = 0; g < ns; ++g) {
+      seb[g] = avg_sub_ebase(eb, S);
+      S += ssum[s0 + g];
+    }
+  }
+  __syncthreads();
+  const int g = t / kAvgHyps, h = t - g * kAvgHyps;
+  if (g < ns) {
+    const int64_t e0 = (s0 + g) * kAvgSub;
+    const AvgHyp r = avg_simulate_hyp(m + e0, (int)min((int64_t)kAvgSub, n - e0), seb[g], h);
+    sh[g][h] = r;
+    srec[s0 + g].h[h] = r;
+    if (h == 0) srec[s0 + g].ebase = seb[g];
+  }
+  __syncthreads();
+  if (t < kAvgHyps) {
+    AvgHyp acc = sh[0][t];
+    for (int k = 1; k < ns; ++k) acc = avg_compose(acc, t & 1, sh[k][t & ~1], sh[k][t | 1]);
+    crec[c].h[t] = acc;
+  }
+}
+
+// the combine walk, one warp: every lane runs the same sequence on the same (shared-memory) values, so the state and the
+// branches are warp-uniform and all lanes help stage the records and data a branch needs
+__global__ void __launch_bounds__(32) avg_walk_kernel(const float *__restrict__ m, int64_t n, const AvgRec *__restrict__ srec,
+                                                      const AvgRec *__restrict__ crec, float *__restrict__ avg) {
+  __shared__ AvgRec cr[32], sr[kAvgGroup];
+  __shared__ float xs[kAvgSub];
+  const int lane = threadIdx.x;
+  const int64_t nsub = ceil_div64(n, kAvgSub);
+  const int nch = (int)ceil_div64(nsub, kAvgGroup);
+  float a = 0.f;
+  for (int c0 = 0; c0 < nch; c0 += 32) {
+    __syncwarp();
+    if (c0 + lane < nch) cr[lane] = crec[c0 + lane];
+    __syncwarp();
+    const int c1 = min(nch, c0 + 32);
+    for (int c = c0; c < c1; ++c) {
+      float j;
+      if (avg_try_jump(a, cr[c - c0], &j)) { a = j; continue; }
+      const int64_t s0 = (int64_t)c * kAvgGroup;
+      const int ns = (int)min((int64_t)kAvgGroup, nsub - s0);
+      __syncwarp();
+      if (lane < ns) sr[lane] = srec[s0 + lane];
+      __syncwarp();
+      for (int g = 0; g < ns; ++g) {
+        if (avg_try_jump(a, sr[g], &j)) { a = j; continue; }
+        const int64_t e0 = (s0 + g) * kAvgSub;
+        const int len = (int)min((int64_t)kAvgSub, n - e0);
+        __syncwarp();
+        for (int i = lane; i < len; i += 32) xs[i] = __ldg(m + e0 + i);
+        __syncwarp();
+#pragma unroll 8
+        for (int i = 0; i < len; ++i) a = __fadd_rn(a, xs[i]);
+      }
+    }
+  }
+  if (lane == 0) *avg = avg_finish(a, n);
+}
+
+static int launch_exact_avg(const float *m, int64_t n, void *ws, float *avg, cudaStream_t st) {
+  const AvgWs w = avg_ws(ws, n);
+  avg_sum_kernel<<<w.nch, 256, 0, st>>>(m, n, w.ssum, w.csum);
+  FAV_TRY(post_launch("avg.sum"));
+  avg_hyp_kernel<<<w.nch, kAvgHypThreads, 0, st>>>(m, n, w.ssum, w.csum, w.srec, w.crec);
+  FAV_TRY(post_launch("avg.hyp"));
+  avg_walk_kernel<<<1, 32, 0, st>>>(m, n, w.srec, w.crec, avg);
+  return post_launch("avg.walk");
+}
+
+// fav_compute_corners with the image planes scaled by `scale` (see structure_tensor_kernel)
+int launch_compute_corners(const float *image, float scale, int Z, int W, int H, float rho, float *corners, float *avg_out,
+                           void *workspace, cudaStream_t st);
 
 }  // namespace fav
 
@@ -348,8 +468,9 @@ int fav_consistency_check(const float *flow1, const float *flow2, const float *s
 size_t fav_compute_corners_workspace(int Z, int W, int H) {
   (void)Z;
   // dxx,dyy,dxy + 3 scratch planes + 3 transposed planes + minmax + the per-block maxima / carries / minima of the normalize scan
+  // + the chunk sums and records of the exact average (launch_exact_avg), after the normalize scan's area
   const size_t nb = ((size_t)W * H + 1023) / 1024;
-  return (size_t)9 * W * H * sizeof(float) + (8 + 3 * nb + 8) * sizeof(float) + 256;  // dxx,dyy,dxy + v1 scratch x3 + transposed x3
+  return (size_t)9 * W * H * sizeof(float) + (8 + 3 * nb + 8) * sizeof(float) + 256 + avg_ws_bytes((int64_t)W * H);
 }
 
 int fav_compute_corners(const float *image, int Z, int W, int H, float rho, float *corners, float *avg_out,
@@ -357,11 +478,16 @@ int fav_compute_corners(const float *image, int Z, int W, int H, float rho, floa
   FAV_REQUIRE(image && corners && workspace, "computeCorners: null tensor");
   FAV_REQUIRE(Z > 0 && W >= 3 && H >= 3, "computeCorners: image too small");
   FAV_TRY(require_device());
-  cudaStream_t st = (cudaStream_t)stream;
+  return launch_compute_corners(image, 1.0f, Z, W, H, rho, corners, avg_out, workspace, (cudaStream_t)stream);
+}
+}
+
+int fav::launch_compute_corners(const float *image, float scale, int Z, int W, int H, float rho, float *corners, float *avg_out,
+                                void *workspace, cudaStream_t st) {
   int64_t n = (int64_t)W * H;
   float *dxx = (float *)workspace, *dyy = dxx + n, *dxy = dyy + n, *scr = dxy + n, *minmax = scr + 6 * n;
   dim3 b2(32, 8), g2(ceil_div(W, 32), ceil_div(H, 8));
-  structure_tensor_kernel<<<g2, b2, 0, st>>>(image, Z, W, H, dxx, dyy, dxy);
+  structure_tensor_kernel<<<g2, b2, 0, st>>>(image, scale, Z, W, H, dxx, dyy, dxy);
   FAV_TRY(post_launch("computeCorners.structure"));
   // coefficients exactly as CFilter.h:1420-1426 (double expressions rounded to float)
   IirC c;
@@ -400,9 +526,8 @@ int fav_compute_corners(const float *image, int Z, int W, int H, float rho, floa
   normalize_apply_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(corners, n, minmax);
   FAV_TRY(post_launch("normalize.apply"));
   if (avg_out) {
-    avg_scan_kernel<<<1, 256, 0, st>>>(corners, n, avg_out);
-    FAV_TRY(post_launch("avg.scan"));
+    const size_t nb = (size_t)ceil_div64(n, kNormBlock);
+    FAV_TRY(launch_exact_avg(corners, n, (char *)(minmax + 8 + 3 * nb + 8) + 256, avg_out, st));
   }
   return FAV_OK;
-}
 }

@@ -348,6 +348,8 @@ __global__ void __launch_bounds__(256) temporal_input_kernel(
 //   1. certainty of the tile + a (r/2)-pixel halo into shared memory: MODE 0 = the occlusion test itself
 //      (consistencyChecker.cpp:99-125, 3-argument mode; flow1 = the backward flow that also drives the warp, flow2 = forward
 //      flow) -- halo pixels are recomputed instead of exchanged; MODE 1 = a given certainty plane (func_load_cert output);
+//      MODE 2 = MODE 0 in 4-argument mode (consistencyChecker.cpp:122-124, makeOptFlow_deepflow.sh:58-60): the structure term
+//      from the corners plane and the device average of fav_compute_corners;
 //   2. utils.min_filter (utils.lua:161-169) as a separable r x r minimum in shared memory (pad cells = +inf);
 //   3. warp + preprocess + mask + concat of the thread's 4 pixels (temporal_pixels above).
 // Bit-identical to consistency_kernel -> min_filter_kernel -> temporal_input_kernel (tests/test_gpu_front.py).
@@ -357,7 +359,8 @@ __global__ void __launch_bounds__(256) temporal_stage_kernel(
     const float *__restrict__ content, const float *__restrict__ prev, const float *__restrict__ flow,
     const float *__restrict__ fw_u, const float *__restrict__ fw_v, const float *__restrict__ cert_raw,
     const float *__restrict__ fill, const float *__restrict__ flow_mask, float *__restrict__ out7,
-    float *__restrict__ cert_out, int H, int W, int r, int border_mode, Operand dst, int R) {
+    float *__restrict__ cert_out, int H, int W, int r, int border_mode, Operand dst, int R,
+    const float *__restrict__ structure, const float *__restrict__ structure_avg) {
   __shared__ float cs[TS_TY + 2 * TS_MAXP][TS_TX + 2 * TS_MAXP + 1];
   __shared__ float rm[TS_TY + 2 * TS_MAXP][TS_TX + 1];
   const int p = r / 2, bx = blockIdx.x * TS_TX, by = blockIdx.y * TS_TY;
@@ -370,7 +373,8 @@ __global__ void __launch_bounds__(256) temporal_stage_kernel(
     cert_out = img_plane(cert_out, b, HW);
     dst = image_of(dst, b);
   }
-  if (MODE == 0) {
+  if (MODE == 0 || MODE == 2) {
+    const float savg = MODE == 2 ? __ldg(structure_avg) : 0.f;
     // kTsBatch pixels per thread and pass: first the (coalesced) backward-flow loads of all of them, then all their forward-flow
     // gathers, then the arithmetic -- up to 8 * kTsBatch loads in flight per thread instead of one pixel's dependent chain
     constexpr int kTsBatch = 3;
@@ -400,7 +404,7 @@ __global__ void __launch_bounds__(256) temporal_stage_kernel(
       for (int k = 0; k < kTsBatch; ++k) {
         if (i0 + k * 256 >= tw * th) break;
         // outside the image: ignored by the max-pooling of utils.min_filter (-inf padding)
-        cs[ty[k]][tx[k]] = in[k] ? (check_eval(t[k], u2[k], v2[k], gx[k], gy[k], W, nullptr, 0.f) ? 1.f : 0.f) : INFINITY;
+        cs[ty[k]][tx[k]] = in[k] ? (check_eval(t[k], u2[k], v2[k], gx[k], gy[k], W, MODE == 2 ? structure : nullptr, savg) ? 1.f : 0.f) : INFINITY;
       }
     }
   } else {
@@ -482,13 +486,27 @@ int launch_temporal_stage(const float *content, const float *prev, const float *
   dim3 grid(ceil_div(W, TS_TX), ceil_div(H, TS_TY), nimg);
   const Operand d = dst ? *dst : Operand();
   if (fw_uv) {
-    if (dst) temporal_stage_kernel<true, 0><<<grid, 256, 0, st>>>(content, prev, flow, fw_uv, fw_uv + HW, nullptr, fill, flow_mask, nullptr, cert_out, H, W, r, border_mode, d, R);
-    else temporal_stage_kernel<false, 0><<<grid, 256, 0, st>>>(content, prev, flow, fw_uv, fw_uv + HW, nullptr, fill, flow_mask, out7, cert_out, H, W, r, border_mode, d, R);
+    if (dst) temporal_stage_kernel<true, 0><<<grid, 256, 0, st>>>(content, prev, flow, fw_uv, fw_uv + HW, nullptr, fill, flow_mask, nullptr, cert_out, H, W, r, border_mode, d, R, nullptr, nullptr);
+    else temporal_stage_kernel<false, 0><<<grid, 256, 0, st>>>(content, prev, flow, fw_uv, fw_uv + HW, nullptr, fill, flow_mask, out7, cert_out, H, W, r, border_mode, d, R, nullptr, nullptr);
   } else {
-    if (dst) temporal_stage_kernel<true, 1><<<grid, 256, 0, st>>>(content, prev, flow, nullptr, nullptr, cert_raw, fill, flow_mask, nullptr, cert_out, H, W, r, border_mode, d, R);
-    else temporal_stage_kernel<false, 1><<<grid, 256, 0, st>>>(content, prev, flow, nullptr, nullptr, cert_raw, fill, flow_mask, out7, cert_out, H, W, r, border_mode, d, R);
+    if (dst) temporal_stage_kernel<true, 1><<<grid, 256, 0, st>>>(content, prev, flow, nullptr, nullptr, cert_raw, fill, flow_mask, nullptr, cert_out, H, W, r, border_mode, d, R, nullptr, nullptr);
+    else temporal_stage_kernel<false, 1><<<grid, 256, 0, st>>>(content, prev, flow, nullptr, nullptr, cert_raw, fill, flow_mask, out7, cert_out, H, W, r, border_mode, d, R, nullptr, nullptr);
   }
   return post_launch("temporal_stage");
+}
+
+// the stage in 4-argument mode (MODE 2), writing the network's first operand; one image
+int launch_temporal_stage_structure(const float *content, const float *prev, const float *flow, const float *fw_uv,
+                                    const float *structure, const float *structure_avg, const float *fill, const float *flow_mask,
+                                    float *cert_out, const Operand &dst, int R, int H, int W, int r, int border_mode, cudaStream_t st) {
+  const bool vec = (W % 4 == 0) && aligned16(content) && aligned16(flow) && (!flow_mask || aligned16(flow_mask)) &&
+                   (!fill || aligned16(fill)) && (!cert_out || aligned16(cert_out));
+  if (!vec || r < 0 || r / 2 > TS_MAXP || (r > 1 && !(r & 1))) return FAV_ERR_UNSUPPORTED;
+  const int64_t HW = (int64_t)H * W;
+  dim3 grid(ceil_div(W, TS_TX), ceil_div(H, TS_TY), 1);
+  temporal_stage_kernel<true, 2><<<grid, 256, 0, st>>>(content, prev, flow, fw_uv, fw_uv + HW, nullptr, fill, flow_mask, nullptr,
+                                                       cert_out, H, W, r, border_mode, dst, R, structure, structure_avg);
+  return post_launch("temporal_stage.structure");
 }
 
 int launch_temporal_input(const float *content, const float *prev, const float *flow, const float *cert,

@@ -29,6 +29,11 @@ int launch_consistency(const float *f1u, const float *f1v, const float *f2u, con
 int launch_temporal_input_packed(const float *content, const float *prev, const float *flow, const float *cert,
                                  const float *fill, const float *flow_mask, const Operand &dst, int R, int H, int W,
                                  int border_mode, bool first, cudaStream_t st, int nimg = 1);
+int launch_temporal_stage_structure(const float *content, const float *prev, const float *flow, const float *fw_uv,
+                                    const float *structure, const float *structure_avg, const float *fill, const float *flow_mask,
+                                    float *cert_out, const Operand &dst, int R, int H, int W, int r, int border_mode, cudaStream_t st);
+int launch_compute_corners(const float *image, float scale, int Z, int W, int H, float rho, float *corners, float *avg_out,
+                           void *workspace, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------------
 struct Param {
@@ -98,6 +103,10 @@ struct Plan {
   float *msb = nullptr;
   float *in7 = nullptr, *out3 = nullptr;  // scratch for run_image / run_next_image
   float *cert_a = nullptr, *cert_b = nullptr;  // scratch of the unfused fallback of fav_run_next_image_flows
+  // 4-argument mode (fav_run_next_image_flows_structure): the corners plane, its average and fav_compute_corners' workspace,
+  // allocated on the first such call
+  float *structure = nullptr, *structure_avg = nullptr;
+  void *corners_ws = nullptr;
   std::vector<PlanStep> steps;
   std::map<int, int> layer_operand;  // arch token index -> operand holding its output
   // CUDA graphs of the whole per-frame kernel sequence (run_[next_]image), one per destination buffer: a frame is ~40
@@ -1016,6 +1025,50 @@ int fav_run_next_image_flows_batch(fav_net_t *net, const float *content, const f
     }
     rc = launch_temporal_input_packed(content, prev_rgb, flow_bw, cert, fill, flow_mask, pl->ops[0], net->reflect_pad, H, W,
                                       border_mode, false, st, B);
+  }
+  FAV_TRY(rc);
+  return run_plan_frame(net, *pl, nullptr, out_rgb, st);
+}
+
+// a-8 in 4-argument mode (makeOptFlow_deepflow.sh:58-60, consistencyChecker.cpp:39-78,122-124,154-160): the certainty of
+// fav_run_next_image_flows with the structure term of the frame being stylized.  `content` is image.load's byte/255, and
+// fl(fl(byte/255) * 255) == byte, so the corners read CTensor's 0..255 planes of the same file.  Per frame: the corners chain,
+// the fused stage (MODE 2), the network's graph launch.
+int fav_run_next_image_flows_structure(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow_bw,
+                                       const float *flow_fw_uv, const float *fill, const float *flow_mask, int H, int W,
+                                       int min_filter_r, int border_mode, float *out_rgb, void *stream) {
+  FAV_REQUIRE(net && content && prev_rgb && flow_bw && flow_fw_uv && out_rgb, "fav_run_next_image_flows_structure: null argument");
+  FAV_REQUIRE(net->finalized, "fav_run_next_image_flows_structure: call fav_net_finalize first");
+  FAV_REQUIRE(net->in_dim == 7, "fav_run_next_image_flows_structure: video model (7 input channels) required");
+  FAV_REQUIRE(H >= 3 && W >= 3, "fav_run_next_image_flows_structure: frame %dx%d below computeCorners' 3x3", W, H);
+  FAV_REQUIRE(border_mode == FAV_BORDER_PER_TAP || border_mode == FAV_BORDER_PAD_PIXEL, "bad border_mode");
+  FAV_REQUIRE(min_filter_r >= 0 && (min_filter_r <= 1 || (min_filter_r & 1)) && min_filter_r <= 15, "occlusions_min_filter must be odd <= 15");
+  Plan *pl;
+  FAV_TRY(build_plan(net, 1, H, W, &pl));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t HW = (int64_t)H * W;
+  if (!pl->corners_ws) {
+    FAV_TRY(alloc_zero(*pl, (void **)&pl->structure, HW * sizeof(float)));
+    FAV_TRY(alloc_zero(*pl, (void **)&pl->structure_avg, 16));
+    FAV_TRY(alloc_zero(*pl, &pl->corners_ws, fav_compute_corners_workspace(3, W, H)));
+  }
+  FAV_TRY(launch_compute_corners(content, 255.0f, 3, W, H, 3.0f, pl->structure, pl->structure_avg, pl->corners_ws, st));
+  int rc = launch_temporal_stage_structure(content, prev_rgb, flow_bw, flow_fw_uv, pl->structure, pl->structure_avg, fill, flow_mask,
+                                           nullptr, pl->ops[0], net->reflect_pad, H, W, min_filter_r, border_mode, st);
+  if (rc == FAV_ERR_UNSUPPORTED) {  // unaligned planes / W % 4 != 0: the three separate kernels
+    if (!pl->cert_a) {
+      FAV_TRY(alloc_zero(*pl, (void **)&pl->cert_a, HW * sizeof(float)));
+      FAV_TRY(alloc_zero(*pl, (void **)&pl->cert_b, HW * sizeof(float)));
+    }
+    FAV_TRY(launch_consistency(flow_bw + HW, flow_bw, flow_fw_uv, flow_fw_uv + HW, pl->structure, pl->structure_avg, 0.f, nullptr,
+                               pl->cert_a, W, H, st));
+    const float *cert = pl->cert_a;
+    if (min_filter_r > 1) {
+      FAV_TRY(launch_min_filter(cert, pl->cert_b, 1, H, W, min_filter_r, st));
+      cert = pl->cert_b;
+    }
+    rc = launch_temporal_input_packed(content, prev_rgb, flow_bw, cert, fill, flow_mask, pl->ops[0], net->reflect_pad, H, W,
+                                      border_mode, false, st);
   }
   FAV_TRY(rc);
   return run_plan_frame(net, *pl, nullptr, out_rgb, st);

@@ -6,10 +6,12 @@
 // double buffered and ordered with events, so copies overlap compute whenever the caller's host buffers are
 // pinned.  Nothing in the loop synchronises the host except fav_session_sync(); host buffers handed to a call must stay
 // untouched until then (the copies are asynchronous).  Per frame the compute stream runs TWO launches: the fused
-// temporal-stage kernel (fav_run_next_image_flows) and the CUDA graph of the network.
+// temporal-stage kernel (fav_run_next_image_flows) and the CUDA graph of the network; the 4-argument variants run the
+// corners chain of fav_compute_corners (structure tensor, transposes, IIRs, eigenvalues, normalize scan, the three kernels
+// of the exact average) before them.
 // The flows variant evaluates checkConsistency in its 3-argument mode (video_dataset/make_occlusions.sh:31-36); the
-// 4-argument structure term of makeOptFlow_deepflow.sh:59-60 is available through fav_compute_corners +
-// fav_consistency_check + the cert-given variant.
+// flows_structure variant in the 4-argument mode of makeOptFlow_deepflow.sh:58-60, with the structure term from the frame
+// being stylized: it adds the corners chain (fav_compute_corners' kernels) before the stage kernel.
 #include <memory>
 #include <vector>
 
@@ -26,7 +28,7 @@ struct fav_session {
   struct InSet {
     float *content = nullptr, *flow = nullptr, *flow_fw = nullptr, *cert_raw = nullptr, *cert = nullptr;
     unsigned char *rgb8 = nullptr, *cert8 = nullptr;  // file payloads (fav_session_run_frame_bytes), allocated on first use
-    float *flo_uv = nullptr;
+    float *flo_uv = nullptr, *flo_fw_uv = nullptr;
     cudaEvent_t uploaded = nullptr, consumed = nullptr;
     bool used = false;
   } in[2];
@@ -54,10 +56,12 @@ namespace {
 // ---- file payloads <-> planes (f-2): what image.load / flowFile.load / image.save do on the host in the reference
 // (fast_artistic_video.lua:95,103,161; flowFileLoader.lua:28-34), moved behind the copy engines.  Same fp32 operations as the
 // host readers of flo_io.cpp and the quantisation of video_pipeline.cu, so files and frames are bit-identical either way.
+// flo_fw (may be NULL): a forward-flow payload, written as the (u, v) planes the occlusion test reads
 __global__ void __launch_bounds__(256) decode_bytes_kernel(const unsigned char *__restrict__ rgb, const float2 *__restrict__ flo,
                                                            const unsigned char *__restrict__ cert8, int invert,
                                                            float *__restrict__ content, float *__restrict__ flow,
-                                                           float *__restrict__ cert, int64_t HW) {
+                                                           float *__restrict__ cert, int64_t HW,
+                                                           const float2 *__restrict__ flo_fw, float *__restrict__ flow_fw) {
   const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
   if (i >= HW) return;
 #pragma unroll
@@ -65,6 +69,10 @@ __global__ void __launch_bounds__(256) decode_bytes_kernel(const unsigned char *
   if (flo) {
     const float2 f = __ldg(flo + i);  // .flo payload: (u, v) pairs; the loader returns [dy = v, dx = u] (flowFileLoader.lua:31-32)
     flow[i] = f.y; flow[HW + i] = f.x;
+  }
+  if (flo_fw) {
+    const float2 f = __ldg(flo_fw + i);
+    flow_fw[i] = f.x; flow_fw[HW + i] = f.y;
   }
   if (cert8) {
     float c = __fdiv_rn((float)cert8[i], 255.0f);
@@ -149,7 +157,7 @@ int fav_session_create(fav_net_t *net, int H, int W, fav_session_t **out) {
   return FAV_OK;
 }
 
-// mode 0: first frame; 1: cert given; 2: cert from the flow pair
+// mode 0: first frame; 1: cert given; 2: cert from the flow pair; 3: cert from the flow pair and the frame (4-argument mode)
 static int session_step(fav_session *s, int mode, const float *content_host, const float *flow_a, const float *flow_b,
                         const float *cert_host, int min_filter_r, int border_mode, float *out_host) {
   FAV_REQUIRE(s && content_host && out_host, "fav_session: null argument");
@@ -165,7 +173,7 @@ static int session_step(fav_session *s, int mode, const float *content_host, con
   if (mode == 1) {
     FAV_TRY(check_cuda(cudaMemcpyAsync(in.flow, flow_a, 2 * HW * 4, cudaMemcpyHostToDevice, s->s_h2d), "H2D flow"));
     FAV_TRY(check_cuda(cudaMemcpyAsync(in.cert_raw, cert_host, HW * 4, cudaMemcpyHostToDevice, s->s_h2d), "H2D cert"));
-  } else if (mode == 2) {
+  } else if (mode >= 2) {
     // backward flow arrives in .flo order (u,v); the warp wants (dy,dx) = (v,u): swap planes while uploading
     FAV_TRY(check_cuda(cudaMemcpyAsync(in.flow + HW, flow_a, HW * 4, cudaMemcpyHostToDevice, s->s_h2d), "H2D flow u"));
     FAV_TRY(check_cuda(cudaMemcpyAsync(in.flow, flow_a + HW, HW * 4, cudaMemcpyHostToDevice, s->s_h2d), "H2D flow v"));
@@ -179,6 +187,9 @@ static int session_step(fav_session *s, int mode, const float *content_host, con
   FAV_TRY(check_cuda(cudaEventRecord(s->t0, s->s_comp), "cudaEventRecord"));
   if (mode == 0) {
     FAV_TRY(fav_run_image(s->net_img ? s->net_img : s->net, in.content, nullptr, H, W, s->out[so], s->s_comp));
+  } else if (mode == 3) {
+    FAV_TRY(fav_run_next_image_flows_structure(s->net, in.content, s->out[so ^ 1], in.flow, in.flow_fw, nullptr, nullptr, H, W,
+                                               min_filter_r, border_mode, s->out[so], s->s_comp));
   } else {
     // ONE temporal-stage kernel per frame: occlusion test (mode 2) or given certainty (mode 1) -> min filter -> warp ->
     // preprocess -> mask -> concat -> first operand of the net; then one graph launch
@@ -223,6 +234,12 @@ int fav_session_run_next_image_flows(fav_session_t *s, const float *content_host
   return session_step(s, 2, content_host, flow_bw_uv_host, flow_fw_uv_host, nullptr, min_filter_r, border_mode, out_host);
 }
 
+int fav_session_run_next_image_flows_structure(fav_session_t *s, const float *content_host, const float *flow_bw_uv_host,
+                                               const float *flow_fw_uv_host, int min_filter_r, int border_mode, float *out_host) {
+  FAV_REQUIRE(flow_bw_uv_host && flow_fw_uv_host, "fav_session_run_next_image_flows_structure: null flow");
+  return session_step(s, 3, content_host, flow_bw_uv_host, flow_fw_uv_host, nullptr, min_filter_r, border_mode, out_host);
+}
+
 // The two conversions as device-pointer entry points (multi-GPU data plane: frames travel as the 8-bit pixels the files hold and
 // are converted on the GPU that owns the clip).  Any of flo_uv / cert8 (and their outputs) may be NULL.
 int fav_bytes_to_planes(const unsigned char *rgb_hwc, const float *flo_uv, const unsigned char *cert8, int invert_occlusion,
@@ -232,7 +249,7 @@ int fav_bytes_to_planes(const unsigned char *rgb_hwc, const float *flo_uv, const
   FAV_TRY(require_device());
   const int64_t HW = (int64_t)H * W;
   decode_bytes_kernel<<<(unsigned)((HW + 255) / 256), 256, 0, (cudaStream_t)stream>>>(rgb_hwc, (const float2 *)flo_uv, cert8, invert_occlusion,
-                                                                                  content, flow, cert, HW);
+                                                                                  content, flow, cert, HW, nullptr, nullptr);
   return post_launch("decode_bytes");
 }
 
@@ -247,10 +264,11 @@ int fav_planes_to_png_rows(const float *rgb_planes, unsigned char *rows, int H, 
 // cert8 = the P5 payload of the certainty (both NULL for the first frame / a single image); png_rows_host receives
 // H*(1+3W) bytes of Sub-filtered PNG scanlines of the stylized frame.  The byte <-> float conversions run on the copy
 // streams (decode after the H2D, encode before the D2H), the compute stream runs exactly what fav_session_run_next_image runs.
-int fav_session_run_frame_bytes(fav_session_t *s, const unsigned char *rgb_hwc, const float *flo_uv, const unsigned char *cert8,
-                                int invert_occlusion, int min_filter_r, int border_mode, unsigned char *png_rows_host) {
-  FAV_REQUIRE(s && rgb_hwc && png_rows_host, "fav_session_run_frame_bytes: null argument");
-  FAV_REQUIRE((flo_uv != nullptr) == (cert8 != nullptr), "fav_session_run_frame_bytes: flow and certainty come together");
+// flo_fw_uv != NULL (cert8 then NULL): the certainty in 4-argument mode from the two flows and the frame
+// (fav_session_run_frame_bytes_flows)
+static int frame_bytes_step(fav_session_t *s, const unsigned char *rgb_hwc, const float *flo_uv, const float *flo_fw_uv,
+                            const unsigned char *cert8, int invert_occlusion, int min_filter_r, int border_mode,
+                            unsigned char *png_rows_host) {
   const bool first = flo_uv == nullptr;
   FAV_REQUIRE(first || s->have_prev, "fav_session_run_frame_bytes: no previous frame");
   FAV_REQUIRE(min_filter_r == 0 || ((min_filter_r & 1) && min_filter_r <= 15), "occlusions_min_filter must be odd <= 15");
@@ -267,16 +285,22 @@ int fav_session_run_frame_bytes(fav_session_t *s, const unsigned char *rgb_hwc, 
       FAV_TRY(s_alloc(s, &s->in[i].flo_uv, 2 * HW));
     }
   }
+  if (flo_fw_uv && !in.flo_fw_uv)
+    for (int i = 0; i < 2; ++i) FAV_TRY(s_alloc(s, &s->in[i].flo_fw_uv, 2 * HW));
   // ---- H2D + decode
   if (in.used) FAV_TRY(check_cuda(cudaStreamWaitEvent(s->s_h2d, in.consumed, 0), "cudaStreamWaitEvent"));
   FAV_TRY(check_cuda(cudaMemcpyAsync(in.rgb8, rgb_hwc, 3 * HW, cudaMemcpyHostToDevice, s->s_h2d), "H2D rgb"));
   if (!first) {
     FAV_TRY(check_cuda(cudaMemcpyAsync(in.flo_uv, flo_uv, 2 * HW * 4, cudaMemcpyHostToDevice, s->s_h2d), "H2D flo"));
-    FAV_TRY(check_cuda(cudaMemcpyAsync(in.cert8, cert8, HW, cudaMemcpyHostToDevice, s->s_h2d), "H2D cert"));
+    if (cert8) FAV_TRY(check_cuda(cudaMemcpyAsync(in.cert8, cert8, HW, cudaMemcpyHostToDevice, s->s_h2d), "H2D cert"));
+    if (flo_fw_uv)
+      FAV_TRY(check_cuda(cudaMemcpyAsync(in.flo_fw_uv, flo_fw_uv, 2 * HW * 4, cudaMemcpyHostToDevice, s->s_h2d), "H2D flo fw"));
   }
   decode_bytes_kernel<<<(unsigned)((HW + 255) / 256), 256, 0, s->s_h2d>>>(in.rgb8, first ? nullptr : (const float2 *)in.flo_uv,
-                                                                        first ? nullptr : in.cert8, invert_occlusion, in.content,
-                                                                        in.flow, in.cert_raw, (int64_t)HW);
+                                                                        cert8 ? in.cert8 : nullptr, invert_occlusion, in.content,
+                                                                        in.flow, in.cert_raw, (int64_t)HW,
+                                                                        flo_fw_uv ? (const float2 *)in.flo_fw_uv : nullptr,
+                                                                        in.flow_fw);
   FAV_TRY(post_launch("decode_bytes"));
   FAV_TRY(check_cuda(cudaEventRecord(in.uploaded, s->s_h2d), "cudaEventRecord"));
   // ---- compute
@@ -285,6 +309,9 @@ int fav_session_run_frame_bytes(fav_session_t *s, const unsigned char *rgb_hwc, 
   FAV_TRY(check_cuda(cudaEventRecord(s->t0, s->s_comp), "cudaEventRecord"));
   if (first) {
     FAV_TRY(fav_run_image(s->net_img ? s->net_img : s->net, in.content, nullptr, H, W, s->out[so], s->s_comp));
+  } else if (flo_fw_uv) {
+    FAV_TRY(fav_run_next_image_flows_structure(s->net, in.content, s->out[so ^ 1], in.flow, in.flow_fw, nullptr, nullptr, H, W,
+                                               min_filter_r, border_mode, s->out[so], s->s_comp));
   } else {
     FAV_TRY(fav_run_next_image_flows(s->net, in.content, s->out[so ^ 1], in.flow, nullptr, in.cert_raw, nullptr, nullptr, H, W,
                                      min_filter_r, border_mode, s->out[so], s->s_comp));
@@ -304,6 +331,20 @@ int fav_session_run_frame_bytes(fav_session_t *s, const unsigned char *rgb_hwc, 
   s->have_prev = true;
   s->frame++;
   return FAV_OK;
+}
+
+int fav_session_run_frame_bytes(fav_session_t *s, const unsigned char *rgb_hwc, const float *flo_uv, const unsigned char *cert8,
+                                int invert_occlusion, int min_filter_r, int border_mode, unsigned char *png_rows_host) {
+  FAV_REQUIRE(s && rgb_hwc && png_rows_host, "fav_session_run_frame_bytes: null argument");
+  FAV_REQUIRE((flo_uv != nullptr) == (cert8 != nullptr), "fav_session_run_frame_bytes: flow and certainty come together");
+  return frame_bytes_step(s, rgb_hwc, flo_uv, nullptr, cert8, invert_occlusion, min_filter_r, border_mode, png_rows_host);
+}
+
+int fav_session_run_frame_bytes_flows(fav_session_t *s, const unsigned char *rgb_hwc, const float *flo_bw_uv,
+                                      const float *flo_fw_uv, int min_filter_r, int border_mode, unsigned char *png_rows_host) {
+  FAV_REQUIRE(s && rgb_hwc && png_rows_host, "fav_session_run_frame_bytes_flows: null argument");
+  FAV_REQUIRE((flo_bw_uv != nullptr) == (flo_fw_uv != nullptr), "fav_session_run_frame_bytes_flows: the two flows come together");
+  return frame_bytes_step(s, rgb_hwc, flo_bw_uv, flo_fw_uv, nullptr, 0, min_filter_r, border_mode, png_rows_host);
 }
 
 // the stylized frame of call number `frame_index` (0-based count of run_* calls on this session) has landed in its out_host

@@ -5,7 +5,9 @@
 //   decoder threads   read the PAYLOADS of frame PPM, certainty PGM and Middlebury .flo straight into PINNED ring slots
 //                     (cudaHostAlloc); byte -> fp32 / 255, 1 - cert, (u,v) -> (dy,dx) planes happen on the GPU behind the H2D
 //                     copy (session.cu: decode_bytes_kernel); the wait-for-file protocol of the flow / occlusion producers
-//                     (utils.lua:74-80) and the [fmt] / {fmt} filename patterns (fast_artistic_video.lua:70-77) are kept
+//                     (utils.lua:74-80) and the [fmt] / {fmt} filename patterns (fast_artistic_video.lua:70-77) are kept;
+//                     fav_video_pipeline_run_flows reads the forward flow instead of the certainty PGM and the certainty is
+//                     the checker's 4-argument mode on the GPU (makeOptFlow_deepflow.sh:58-60)
 //   calling thread    only enqueues frames on the session (3 CUDA streams inside: H2D / compute / D2H)
 //   completer thread  waits for the session's per-frame completion events in order (fav_session_frame_done)
 //   encoder threads   deflate the landed Sub-filtered scanlines (quantised like image.save -- clamp, x255, round -- on the GPU
@@ -148,7 +150,7 @@ inline double now_s() { return std::chrono::duration<double>(std::chrono::steady
 
 struct Slot {  // pinned; file payloads in, PNG scanlines out (the byte <-> float conversions happen on the GPU)
   unsigned char *rgb = nullptr, *cert = nullptr, *rows = nullptr;
-  float *flo = nullptr;
+  float *flo = nullptr, *flo_fw = nullptr;
 };
 
 }  // namespace
@@ -192,13 +194,13 @@ int fav_png_write(const char *path, const unsigned char *pixels, int W, int H, i
 
 // Runs the whole clip; blocks until the last PNG is on disk.  Frames are <input_pattern % i>, i = 1..; the loop ends at
 // num_frames or at the first missing frame file (func_load_image returning nil, fast_artistic_video.lua:93-97).
-// frames_done / seconds (may be NULL) report what was processed.
-int fav_video_pipeline_run(fav_session_t *sess, int H, int W, const char *input_pattern, const char *flow_pattern,
-                           const char *occlusions_pattern, const char *output_prefix, int num_frames, int min_filter_r,
-                           int invert_occlusion, int n_decode, int n_encode, int depth, int png_level, int *frames_done,
-                           double *seconds) {
-  FAV_REQUIRE(sess && input_pattern && flow_pattern && occlusions_pattern && output_prefix, "fav_video_pipeline_run: null argument");
-  FAV_REQUIRE(H > 0 && W > 0 && num_frames >= 0, "fav_video_pipeline_run: bad size");
+// frames_done / seconds (may be NULL) report what was processed.  Exactly one of occlusions_pattern (certainty PGMs) and
+// flow_fw_pattern (forward flows: the certainty is computed from the two flows and the frame) is non-NULL.
+static int pipeline_run(fav_session_t *sess, int H, int W, const char *input_pattern, const char *flow_pattern,
+                        const char *occlusions_pattern, const char *flow_fw_pattern, const char *output_prefix, int num_frames,
+                        int min_filter_r, int invert_occlusion, int n_decode, int n_encode, int depth, int png_level,
+                        int *frames_done, double *seconds) {
+  const bool flows = flow_fw_pattern != nullptr;
   n_decode = n_decode < 1 ? 1 : n_decode; n_encode = n_encode < 1 ? 1 : n_encode;
   depth = depth < 4 ? 4 : (depth > 60 ? 60 : depth);  // <= the session's ring of 64 per-frame completion events
   png_level = png_level < 0 ? 1 : (png_level > 9 ? 9 : png_level);
@@ -211,11 +213,12 @@ int fav_video_pipeline_run(fav_session_t *sess, int H, int W, const char *input_
   std::vector<Slot> slots(depth);
   const size_t row_bytes = (size_t)H * (1 + 3 * (size_t)W);
   auto free_slots = [&]() {
-    for (Slot &s : slots) { cudaFreeHost(s.rgb); cudaFreeHost(s.flo); cudaFreeHost(s.cert); cudaFreeHost(s.rows); }
+    for (Slot &s : slots) { cudaFreeHost(s.rgb); cudaFreeHost(s.flo); cudaFreeHost(s.flo_fw); cudaFreeHost(s.cert); cudaFreeHost(s.rows); }
   };
   for (Slot &s : slots)
     if (cudaHostAlloc((void **)&s.rgb, 3 * HW, cudaHostAllocDefault) != cudaSuccess ||
         cudaHostAlloc((void **)&s.flo, 2 * HW * 4, cudaHostAllocDefault) != cudaSuccess ||
+        (flows && cudaHostAlloc((void **)&s.flo_fw, 2 * HW * 4, cudaHostAllocDefault) != cudaSuccess) ||
         cudaHostAlloc((void **)&s.cert, HW, cudaHostAllocDefault) != cudaSuccess ||
         cudaHostAlloc((void **)&s.rows, row_bytes, cudaHostAllocDefault) != cudaSuccess) {
       (void)cudaGetLastError();
@@ -244,7 +247,8 @@ int fav_video_pipeline_run(fav_session_t *sess, int H, int W, const char *input_
     std::this_thread::sleep_for(std::chrono::seconds(1));
     return true;
   };
-  const std::string in_pat(input_pattern), flow_pat(flow_pattern), occ_pat(occlusions_pattern), out_prefix(output_prefix);
+  const std::string in_pat(input_pattern), flow_pat(flow_pattern), occ_pat(flows ? "" : occlusions_pattern),
+      fw_pat(flows ? flow_fw_pattern : ""), out_prefix(output_prefix);
 
   std::atomic<long long> t_decode{0}, t_png{0}, t_enc_wait{0}, t_dec_wait{0}, t_enq_wait{0};  // microseconds, all threads
   auto us = [](double a, double b) { return (long long)((b - a) * 1e6); };
@@ -264,7 +268,18 @@ int fav_video_pipeline_run(fav_session_t *sess, int H, int W, const char *input_
       const std::string frame_name = format_index(in_pat, i);
       int rc = fav_pnm_read_u8(frame_name.c_str(), s.rgb, 3 * HW, &w, &h, &c);
       if (rc == FAV_OK && (w != W || h != H || c != 3)) { fail(FAV_ERR_IO, frame_name + ": not a " + std::to_string(W) + "x" + std::to_string(H) + " P6 image"); return; }
-      if (rc == FAV_OK && i > 1) {
+      if (rc == FAV_OK && i > 1 && flows) {
+        // makeOptFlow_deepflow.sh:51-58 writes the forward flow last (in the background) and waits for it before the checker
+        const std::string fw_name = format_flow_name(fw_pat, i - 1, i), flow_name = format_flow_name(flow_pat, i - 1, i);
+        if (!wait_for_file(fw_name)) return;
+        rc = fav_flo_read_raw(fw_name.c_str(), s.flo_fw, 2 * HW, &w, &h);
+        if (rc == FAV_OK && (w != W || h != H)) { fail(FAV_ERR_IO, fw_name + ": size mismatch"); return; }
+        if (rc == FAV_OK) {
+          if (!wait_for_file(flow_name)) return;
+          rc = fav_flo_read_raw(flow_name.c_str(), s.flo, 2 * HW, &w, &h);
+          if (rc == FAV_OK && (w != W || h != H)) { fail(FAV_ERR_IO, flow_name + ": size mismatch"); return; }
+        }
+      } else if (rc == FAV_OK && i > 1) {
         const std::string cert_name = format_flow_name(occ_pat, i - 1, i), flow_name = format_flow_name(flow_pat, i - 1, i);
         if (!wait_for_file(cert_name)) return;  // func_load_cert :99-103
         rc = fav_pnm_read_u8(cert_name.c_str(), s.cert, HW, &w, &h, &c);
@@ -331,8 +346,10 @@ int fav_video_pipeline_run(fav_session_t *sess, int H, int W, const char *input_
       if (err != FAV_OK) break;
     }
     Slot &s = slots[(i - 1) % depth];
-    const int rc = fav_session_run_frame_bytes(sess, s.rgb, i == 1 ? nullptr : s.flo, i == 1 ? nullptr : s.cert, invert_occlusion,
-                                               min_filter_r, FAV_BORDER_PER_TAP, s.rows);
+    const int rc = flows ? fav_session_run_frame_bytes_flows(sess, s.rgb, i == 1 ? nullptr : s.flo, i == 1 ? nullptr : s.flo_fw,
+                                                             min_filter_r, FAV_BORDER_PER_TAP, s.rows)
+                         : fav_session_run_frame_bytes(sess, s.rgb, i == 1 ? nullptr : s.flo, i == 1 ? nullptr : s.cert,
+                                                       invert_occlusion, min_filter_r, FAV_BORDER_PER_TAP, s.rows);
     if (rc != FAV_OK) { fail(rc, fav_last_error()); break; }
     { std::lock_guard<std::mutex> lk(mu); ready[i] = 2; }
     cv_enq.notify_all();
@@ -350,5 +367,24 @@ int fav_video_pipeline_run(fav_session_t *sess, int H, int W, const char *input_
             t_enq_wait / 1e3 / n, n_decode, n_encode, depth, png_level);
   if (err != FAV_OK) { set_error("fav_video_pipeline_run: %s", err_msg.c_str()); return err; }
   return FAV_OK;
+}
+
+int fav_video_pipeline_run(fav_session_t *sess, int H, int W, const char *input_pattern, const char *flow_pattern,
+                           const char *occlusions_pattern, const char *output_prefix, int num_frames, int min_filter_r,
+                           int invert_occlusion, int n_decode, int n_encode, int depth, int png_level, int *frames_done,
+                           double *seconds) {
+  FAV_REQUIRE(sess && input_pattern && flow_pattern && occlusions_pattern && output_prefix, "fav_video_pipeline_run: null argument");
+  FAV_REQUIRE(H > 0 && W > 0 && num_frames >= 0, "fav_video_pipeline_run: bad size");
+  return pipeline_run(sess, H, W, input_pattern, flow_pattern, occlusions_pattern, nullptr, output_prefix, num_frames, min_filter_r,
+                      invert_occlusion, n_decode, n_encode, depth, png_level, frames_done, seconds);
+}
+
+int fav_video_pipeline_run_flows(fav_session_t *sess, int H, int W, const char *input_pattern, const char *flow_pattern,
+                                 const char *flow_fw_pattern, const char *output_prefix, int num_frames, int min_filter_r,
+                                 int n_decode, int n_encode, int depth, int png_level, int *frames_done, double *seconds) {
+  FAV_REQUIRE(sess && input_pattern && flow_pattern && flow_fw_pattern && output_prefix, "fav_video_pipeline_run_flows: null argument");
+  FAV_REQUIRE(H > 0 && W > 0 && num_frames >= 0, "fav_video_pipeline_run_flows: bad size");
+  return pipeline_run(sess, H, W, input_pattern, flow_pattern, nullptr, flow_fw_pattern, output_prefix, num_frames, min_filter_r, 0,
+                      n_decode, n_encode, depth, png_level, frames_done, seconds);
 }
 }

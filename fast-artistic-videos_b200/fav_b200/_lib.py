@@ -113,10 +113,18 @@ SIGNATURES = {
     "fav_session_run_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "fav_session_run_next_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "fav_session_run_next_image_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "fav_run_next_image_flows_structure": (C.c_int, [C.c_void_p, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                     _fp, _fp]),
+    "fav_session_run_next_image_flows_structure": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                             C.c_void_p]),
     "fav_session_frame_done": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int]),
     "fav_session_run_frame_bytes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "fav_video_pipeline_run": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.c_int,
                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_double)]),
+    "fav_session_run_frame_bytes_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "fav_video_pipeline_run_flows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int,
+                                               C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                               C.POINTER(C.c_double)]),
     "fav_session_sync": (C.c_int, [C.c_void_p]),
     "fav_session_last_gpu_ms": (C.c_float, [C.c_void_p]),
 }

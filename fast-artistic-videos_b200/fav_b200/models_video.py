@@ -164,6 +164,21 @@ class StyleNet:
                                                                _lib.stream_ptr()))
         return out
 
+    def run_next_image_flows_structure(self, img, prev_rgb, flow_bw, flow_fw_uv, min_filter_r=7, fill=None, flow_mask=None,
+                                       border_mode=_lib.BORDER_PER_TAP) -> torch.Tensor:
+        """run_next_image_flows with the certainty in the checker's 4-argument mode, as the stylization scripts compute it
+        (makeOptFlow_deepflow.sh:58-60): the structure term comes from img [3,H,W] (byte/255 values), the frame being stylized.
+        flow_bw [2,H,W] (dy,dx), flow_fw_uv [2,H,W] (u,v).  One image."""
+        x = img.contiguous()
+        assert x.dim() == 3, "run_next_image_flows_structure: one image [3,H,W]"
+        H, W = x.shape[-2:]
+        out = torch.empty_like(x)
+        p, f, fw = prev_rgb.contiguous(), flow_bw.contiguous(), flow_fw_uv.contiguous()
+        _lib.check(_lib.lib.fav_run_next_image_flows_structure(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(fw),
+                                                               _lib.dptr(fill), _lib.dptr(flow_mask), H, W, int(min_filter_r),
+                                                               border_mode, _lib.dptr(out), _lib.stream_ptr()))
+        return out
+
 
 def _planes(t, img, c):
     """t (or None) as a contiguous tensor of `c` planes per image of the batch img [B,3,H,W]; c = 0: one plane without a

@@ -49,6 +49,13 @@ class Session:
                                                              _hp(flow_fw_uv_host), int(min_filter_r), border_mode,
                                                              _hp(out_host)))
 
+    def run_next_image_flows_structure(self, content_host, flow_bw_uv_host, flow_fw_uv_host, out_host, min_filter_r=7,
+                                       border_mode=_lib.BORDER_PER_TAP):
+        """run_next_image_flows with the certainty in the checker's 4-argument mode (structure term from the frame)."""
+        _lib.check(_lib.lib.fav_session_run_next_image_flows_structure(self._h, _hp(content_host), _hp(flow_bw_uv_host),
+                                                                       _hp(flow_fw_uv_host), int(min_filter_r), border_mode,
+                                                                       _hp(out_host)))
+
     def run_frame_bytes(self, rgb_hwc, flo_uv, cert8, rows_out, invert_occlusion=False, min_filter_r=7,
                         border_mode=_lib.BORDER_PER_TAP):
         """One frame from file payloads (uint8 HWC frame, float32 [H,W,2] (u,v) flow, uint8 certainty; the last two None for
@@ -56,6 +63,13 @@ class Session:
         bp = lambda a: None if a is None else C.c_void_p(a.data_ptr() if isinstance(a, torch.Tensor) else a.ctypes.data)
         _lib.check(_lib.lib.fav_session_run_frame_bytes(self._h, bp(rgb_hwc), bp(flo_uv), bp(cert8), 1 if invert_occlusion else 0,
                                                         int(min_filter_r), border_mode, bp(rows_out)))
+
+    def run_frame_bytes_flows(self, rgb_hwc, flo_bw_uv, flo_fw_uv, rows_out, min_filter_r=7, border_mode=_lib.BORDER_PER_TAP):
+        """run_frame_bytes with the backward and forward .flo payloads (float32 [H,W,2] (u,v); both None for the first frame)
+        instead of a certainty: the certainty is the checker's 4-argument mode with this frame, computed on the GPU."""
+        bp = lambda a: None if a is None else C.c_void_p(a.data_ptr() if isinstance(a, torch.Tensor) else a.ctypes.data)
+        _lib.check(_lib.lib.fav_session_run_frame_bytes_flows(self._h, bp(rgb_hwc), bp(flo_bw_uv), bp(flo_fw_uv), int(min_filter_r),
+                                                              border_mode, bp(rows_out)))
 
     def frame_done(self, frame_index: int, wait: bool = True) -> bool:
         """The output of the frame_index-th run_* call (0-based) has landed in its host buffer."""

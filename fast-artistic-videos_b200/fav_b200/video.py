@@ -14,7 +14,7 @@ import sys
 import numpy as np
 import torch
 
-from . import _lib, core, flowFileLoader, utils
+from . import _lib, consistencyChecker, core, flowFileLoader, utils
 
 
 def build_parser():
@@ -24,6 +24,9 @@ def build_parser():
     a("-num_frames", type=int, default=9999); a("-continue_with", type=int, default=1)
     a("-input_pattern", default=""); a("-output_prefix", default="out")
     a("-flow_pattern", default=""); a("-occlusions_pattern", default="")
+    # forward flows, e.g. forward_{%d}_[%d].flo: with an empty -occlusions_pattern the certainty of frame i is computed on the GPU
+    # from backward_i_{i-1}, forward_{i-1}_i and frame i, as makeOptFlow_deepflow.sh:58-60 computes reliable_i_{i-1}.pgm
+    a("-flow_pattern_forward", default="")
     a("-invert_occlusion", action="store_true"); a("-occlusions_min_filter", type=int, default=7)
     a("-fill_occlusions", default="vgg-mean"); a("-fix_occlusions", action="store_true")
     a("-median_filter", type=int, default=3)  # declared but unused by the plain driver (fast_artistic_video.lua:39)
@@ -128,9 +131,17 @@ class Driver:
 
     def func_load_cert(self, opt, i, dtype):  # :99-112
         flowFileName = getFormatedFlowFileName(opt.flow_pattern, i - 1, i)
-        certFileName = getFormatedFlowFileName(opt.occlusions_pattern, i - 1, i)
-        utils.wait_for_file(certFileName)
-        cert = load_image(certFileName, 1).cuda()
+        if opt.flow_pattern_forward:  # the checker's 4-argument mode on frame i (loaded just before by func_load_image)
+            fwFileName = getFormatedFlowFileName(opt.flow_pattern_forward, i - 1, i)
+            utils.wait_for_file(fwFileName)
+            utils.wait_for_file(flowFileName)
+            bw = torch.from_numpy(flowFileLoader.load(flowFileName, layout=1)).cuda()
+            fw = torch.from_numpy(flowFileLoader.load(fwFileName, layout=1)).cuda()
+            cert = consistencyChecker.check(bw, fw, self.last_frame.cuda() * 255.0, want_cert=True)[1][None]
+        else:
+            certFileName = getFormatedFlowFileName(opt.occlusions_pattern, i - 1, i)
+            utils.wait_for_file(certFileName)
+            cert = load_image(certFileName, 1).cuda()
         if opt.invert_occlusion:
             cert = 1.0 - cert
         if opt.fix_occlusions:
@@ -215,7 +226,8 @@ def pipeline_eligible(opt) -> bool:
 def _native_ok(opt) -> bool:
     """the native pipeline decodes binary PPM / PGM only (what the reference's scripts extract with ffmpeg,
     stylizeVideo_*.sh: frame_%04d.ppm, and what consistencyChecker writes)"""
-    return opt.input_pattern.lower().endswith(".ppm") and opt.occlusions_pattern.lower().endswith(".pgm")
+    return opt.input_pattern.lower().endswith(".ppm") and (opt.flow_pattern_forward != ""
+                                                           or opt.occlusions_pattern.lower().endswith(".pgm"))
 
 
 def run_native(opt, model_vid=None, model_img=None, n_decode=None, n_encode=None, depth=None, png_level=1):
@@ -245,10 +257,16 @@ def run_native(opt, model_vid=None, model_img=None, n_decode=None, n_encode=None
     n_encode = n_encode or max(4, min(64, cpus // 2))
     depth = depth or (n_decode + n_encode + 4)
     nfr, secs = C.c_int(), C.c_double()
-    _lib.check(_lib.lib.fav_video_pipeline_run(sess._h, H, W, opt.input_pattern.encode(), opt.flow_pattern.encode(),
-                                               opt.occlusions_pattern.encode(), opt.output_prefix.encode(), int(opt.num_frames),
-                                               int(opt.occlusions_min_filter), 1 if opt.invert_occlusion else 0, n_decode, n_encode,
-                                               depth, png_level, C.byref(nfr), C.byref(secs)))
+    if opt.flow_pattern_forward:
+        _lib.check(_lib.lib.fav_video_pipeline_run_flows(sess._h, H, W, opt.input_pattern.encode(), opt.flow_pattern.encode(),
+                                                         opt.flow_pattern_forward.encode(), opt.output_prefix.encode(),
+                                                         int(opt.num_frames), int(opt.occlusions_min_filter), n_decode, n_encode,
+                                                         depth, png_level, C.byref(nfr), C.byref(secs)))
+    else:
+        _lib.check(_lib.lib.fav_video_pipeline_run(sess._h, H, W, opt.input_pattern.encode(), opt.flow_pattern.encode(),
+                                                   opt.occlusions_pattern.encode(), opt.output_prefix.encode(), int(opt.num_frames),
+                                                   int(opt.occlusions_min_filter), 1 if opt.invert_occlusion else 0, n_decode,
+                                                   n_encode, depth, png_level, C.byref(nfr), C.byref(secs)))
     if nfr.value:
         print("Stylized %d frames in %.3f s (%.1f frames/s, files -> PNG, native pipeline)" % (nfr.value, secs.value, nfr.value / secs.value))
     return dict(frames=nfr.value, seconds=secs.value)
@@ -334,10 +352,20 @@ def main(argv=None):
     opt = build_parser().parse_args(argv)
     if opt.input_pattern == "":
         raise SystemExit("Must give -input_pattern")  # :177-179
-    if not opt.create_inconsistent and (opt.flow_pattern == "" or opt.occlusions_pattern == ""):
+    if opt.flow_pattern_forward:  # certainties computed from the flow pair and the frame (4-argument checker)
+        if opt.flow_pattern == "":
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, "-flow_pattern_forward needs -flow_pattern (the backward flows)")
+        if opt.occlusions_pattern != "":
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, "give either -occlusions_pattern or -flow_pattern_forward")
+        if opt.invert_occlusion:
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, "-invert_occlusion inverts loaded PGMs; the computed certainty is not inverted")
+    elif not opt.create_inconsistent and (opt.flow_pattern == "" or opt.occlusions_pattern == ""):
         raise SystemExit("Must give -flow_pattern and -occlusions_pattern")  # :180-182
     if opt.pipeline and pipeline_eligible(opt):
-        return run_native(opt) if _native_ok(opt) else run_pipelined(opt)
+        if _native_ok(opt):
+            return run_native(opt)
+        if not opt.flow_pattern_forward:  # the Python pipeline reads certainty PGMs; computed ones take the driver below
+            return run_pipelined(opt)
     d = Driver(opt)
     core.run_fast_neural_video(opt, d.func_load_image, d.func_load_cert, d.func_eval, d.func_make_last_frame_warped,
                                d.func_is_single_image, d.func_save_image)

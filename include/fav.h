@@ -293,6 +293,15 @@ FAV_API int fav_run_next_image_flows(fav_net_t *net, const float *content, const
                                      const float *flow_fw_uv, const float *cert_raw, const float *fill,
                                      const float *flow_mask, int H, int W, int min_filter_r, int border_mode,
                                      float *out_rgb, void *stream);
+/* fav_run_next_image_flows with the certainty in the 4-argument mode of the stylization scripts (makeOptFlow_deepflow.sh:58-60;
+ * consistencyChecker.cpp:39-78,122-124,154-160; read as reliable_[i]_{i-1}.pgm by fast_artistic_video.lua:99-112): the
+ * structure term comes from `content` (byte/255 planes of frame i, the image of the checker's call), flow_bw = [dy,dx] of
+ * backward_i_{i-1}.flo, flow_fw_uv = forward_{i-1}_i.flo in (u,v) order.  The corners, their exact average and the fused
+ * stage run on the device.  One image; H, W >= 3. */
+FAV_API int fav_run_next_image_flows_structure(fav_net_t *net, const float *content, const float *prev_rgb,
+                                               const float *flow_bw, const float *flow_fw_uv, const float *fill,
+                                               const float *flow_mask, int H, int W, int min_filter_r, int border_mode,
+                                               float *out_rgb, void *stream);
 
 /* Batched frame calls (see fav_net_forward_batch): every plane argument holds B images one after the other -- content,
  * prev_rgb, fill, out_rgb [B,3,H,W]; flow, flow_bw, flow_fw_uv [B,2,H,W]; cert, cert_raw, flow_mask [B,H,W].  Each image keeps
@@ -336,6 +345,11 @@ FAV_API int fav_session_run_next_image_flows(fav_session_t *s, const float *cont
                                              const float *flow_bw_uv_host,
                                              const float *flow_fw_uv_host, int min_filter_r,
                                              int border_mode, float *out_host);
+/* same in the checker's 4-argument mode, the structure term from the frame itself (fav_run_next_image_flows_structure;
+ * makeOptFlow_deepflow.sh:58-60, consistencyChecker.cpp:39-78,122-124,154-160). */
+FAV_API int fav_session_run_next_image_flows_structure(fav_session_t *s, const float *content_host,
+                                                       const float *flow_bw_uv_host, const float *flow_fw_uv_host,
+                                                       int min_filter_r, int border_mode, float *out_host);
 /* completion of ONE frame: call number frame_index (0-based) of fav_session_run_* on this session has landed in its out_host
  * buffer (wait != 0 blocks; wait == 0 polls: FAV_OK / FAV_ERR_INVALID "still in flight").  Lets encoder threads consume
  * frames while later ones are still being enqueued (file-driven pipeline, fav_b200/video.py). */
@@ -360,6 +374,12 @@ FAV_API int fav_planes_to_png_rows(const float *rgb_planes, unsigned char *rows,
 FAV_API int fav_session_run_frame_bytes(fav_session_t *s, const unsigned char *rgb_hwc, const float *flo_uv,
                                         const unsigned char *cert8, int invert_occlusion, int min_filter_r, int border_mode,
                                         unsigned char *png_rows_host);
+/* the same with both .flo payloads and no PGM: flo_bw_uv = backward_i_{i-1}.flo, flo_fw_uv = forward_{i-1}_i.flo (both NULL for
+ * the first frame); the certainty is the checker's 4-argument mode with frame i as the image, computed on the GPU as
+ * fav_session_run_next_image_flows_structure does (makeOptFlow_deepflow.sh:58-60, consistencyChecker.cpp:39-78,122-124,154-160). */
+FAV_API int fav_session_run_frame_bytes_flows(fav_session_t *s, const unsigned char *rgb_hwc, const float *flo_bw_uv,
+                                              const float *flo_fw_uv, int min_filter_r, int border_mode,
+                                              unsigned char *png_rows_host);
 /* f-2  the file-driven frame loop (fast_artistic_video.lua:93-170) as a native pipeline around this session: decoder threads
  * (frame PPM, certainty PGM, .flo -> pinned ring slots; [fmt]/{fmt} patterns :70-77; wait-for-file protocol utils.lua:74-80),
  * the calling thread enqueues frames, encoder threads wait per frame and write "<output_prefix>-%05d.png" (:161; zlib level
@@ -369,6 +389,12 @@ FAV_API int fav_video_pipeline_run(fav_session_t *s, int H, int W, const char *i
                                    const char *occlusions_pattern, const char *output_prefix, int num_frames, int min_filter_r,
                                    int invert_occlusion, int n_decode, int n_encode, int depth, int png_level, int *frames_done,
                                    double *seconds);
+/* fav_video_pipeline_run without certainty PGMs: the decoder threads read the backward flow (flow_pattern) and the forward flow
+ * (flow_fw_pattern, e.g. "forward_{%d}_[%d].flo"), waiting for the forward flow first as makeOptFlow_deepflow.sh:58 does, and
+ * each frame runs fav_session_run_frame_bytes_flows (the checker's 4-argument mode on the GPU). */
+FAV_API int fav_video_pipeline_run_flows(fav_session_t *s, int H, int W, const char *input_pattern, const char *flow_pattern,
+                                         const char *flow_fw_pattern, const char *output_prefix, int num_frames, int min_filter_r,
+                                         int n_decode, int n_encode, int depth, int png_level, int *frames_done, double *seconds);
 /* block until every queued frame has landed in its out_host buffer */
 FAV_API int fav_session_sync(fav_session_t *s);
 /* device time (ms, CUDA events on the compute stream) of the last frame's GPU work */
