@@ -73,6 +73,13 @@ static constexpr int kChunkCapBytes = 24 * 1024;
 static constexpr bool kPlanRowFold = false, kPlanPhaseFold = false;
 
 static inline int build_phase_tables(const ConvDef &c, ConvPhase &ph) {
+  // a transposed conv whose stride exceeds its kernel (f1s2) leaves sub-pixel phases that only receive the bias: no K steps to
+  // plan, and no released model has one
+  if (ph.taps.empty()) {
+    set_error("conv %s: sub-pixel phase (%d,%d) without filter taps (kernel %d smaller than stride %d)", c.name.c_str(),
+              ph.oy_off, ph.ox_off, c.k, c.stride);
+    return FAV_ERR_UNSUPPORTED;
+  }
   ph.rows.clear();
   ph.dxmin = 1 << 30; ph.dxmax = -(1 << 30);
   for (auto &t : ph.taps) {

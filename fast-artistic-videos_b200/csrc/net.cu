@@ -390,8 +390,8 @@ static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
   auto it = net->plans.find(key);
   if (it != net->plans.end()) { *out = it->second.get(); net->last_plan = *out; return FAV_OK; }
   if (H % 4 || W % 4 || H < 16 || W < 16) {
-    set_error("frame size %dx%d: H and W must be multiples of 4 (reflect-start nets restore the input size only "
-              "then, SURVEY appendix B)", W, H);
+    set_error("frame size %dx%d: H and W must be multiples of 4 and at least 16 (the default arch's two stride-2 layers "
+              "restore the input size only then, SURVEY appendix B)", W, H);
     return FAV_ERR_INVALID;
   }
   std::unique_ptr<Plan> pl(new Plan());
@@ -414,6 +414,15 @@ static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
         h = ho; w = wo;
         if (op.inorm[i] >= 0 && !net->bn) stats_slots += 2 * c.cout;
       }
+    }
+    // the final conv writes a [3][H][W] frame per image: a net that returns another size would write past it (and into the
+    // next image of a batch).  Every stride-2 layer needs an even input to be undone exactly by the upsampling layers.
+    if (h != H || w != W) {
+      int n2 = 0;
+      for (const ConvDef &c : net->convs) n2 += c.in_stride == 2;
+      set_error("frame size %dx%d: this arch would return a %dx%d frame; with its %d stride-2 layers H and W must be "
+                "multiples of %d (when its residual blocks sit at the lowest resolution)", W, H, w, h, n2, 1 << n2);
+      return FAV_ERR_INVALID;
     }
   }
   pl->raw_bytes = raw_max * sizeof(float) + 4096;  // per image (a multiple of 16 bytes)

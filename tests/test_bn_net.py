@@ -11,11 +11,15 @@ import pytest
 from conftest import ROOT
 
 from fav_b200 import synth
+from test_gpu_arch_geometry import BN_ROWS as GEOMETRY_BN_ROWS, ROWS as GEOMETRY_ROWS
 
 EMU = os.path.join(ROOT, "tests", "emu")
 PAPER = synth.PAPER_ARCH
 WIDE = "c9s1-32,d64,d256,C256,f3s1-192,u96,u32,c9s1-3"
-ARCHS = [(synth.DEFAULT_ARCH, "reflect-start"), (synth.DEFAULT_ARCH, "zero"), (PAPER, "reflect-start"), (WIDE, "reflect-start")]
+# + the BN rows of the arch-geometry table: epilogues writing operands with padT 3 / 4 (c7s1 / c9s1 consumers) and tpad 2 - 4
+# (f5s1 / f7s1 / f9s1 consumers)
+ARCHS = [(synth.DEFAULT_ARCH, "reflect-start"), (synth.DEFAULT_ARCH, "zero"), (PAPER, "reflect-start"), (WIDE, "reflect-start")] + \
+    [GEOMETRY_ROWS[name][:2] for name in GEOMETRY_BN_ROWS]
 
 
 def _write_read(tmp_path, arch, w, **kw):

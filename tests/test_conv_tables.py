@@ -52,6 +52,30 @@ CASES = [  # cin, cout, k, stride, pad, transposed, adj, H, W
     (8, 3, 9, 1, 4, 0, 0, 6, 140),       # final conv from 8 channels: tap pairing, plain final epilogue
     (32, 3, 3, 1, 1, 0, 0, 5, 129),      # final c3s1-3: generic plan, plain final epilogue
     (32, 8, 3, 2, 1, 1, 1, 4, 70),       # u8: Cout 8 in an N = 16 instance
+    # first conv (tap pairing) at k 1 / 3 / 5 / 7, from 7 and from 3 channels
+    (7, 32, 1, 1, 0, 0, 0, 6, 140),
+    (7, 32, 3, 1, 1, 0, 0, 6, 140),
+    (7, 32, 5, 1, 2, 0, 0, 6, 140),
+    (7, 32, 7, 1, 3, 0, 0, 6, 140),
+    (3, 32, 7, 1, 3, 0, 0, 6, 140),
+    # non-final stride-1 convs: c1s1 from 32, c5s1 from 32 (two A stages, 223 KB of shared memory), c7s1 from 64, c9s1 from 16
+    (32, 64, 1, 1, 0, 0, 0, 5, 130),
+    (32, 64, 5, 1, 2, 0, 0, 6, 130),
+    (64, 64, 7, 1, 3, 0, 0, 8, 130),
+    (16, 32, 9, 1, 4, 0, 0, 10, 130),
+    # final convs: x-fold c7s1-3 (122-px tile stride, 3 tiles, the last 1 pixel wide), generic c1s1-3, tap-paired c5s1-3
+    (32, 3, 7, 1, 3, 0, 0, 8, 245),
+    (32, 3, 1, 1, 0, 0, 0, 5, 130),
+    (8, 3, 5, 1, 2, 0, 0, 6, 130),
+    # stride-1 transposed convs f1s1 / f5s1 / f7s1 / f9s1: the flipped filter on an operand with a zero border of tpad 0 - 4
+    (32, 32, 1, 1, 0, 1, 0, 5, 130),
+    (32, 32, 5, 1, 2, 1, 0, 6, 130),
+    (32, 32, 7, 1, 3, 1, 0, 6, 130),
+    (32, 16, 9, 1, 4, 1, 0, 6, 130),
+    # stride-2 transposed convs: f7s2 (phases with 16/12/12/9 taps, tpad 1), f9s2 (25/20/20/16, tpad 2), u16 from 8 channels
+    (64, 32, 7, 2, 3, 1, 1, 5, 70),
+    (64, 32, 9, 2, 4, 1, 1, 5, 70),
+    (8, 16, 3, 2, 1, 1, 1, 4, 70),
 ]
 
 
@@ -62,6 +86,15 @@ def test_emulated_kernel_addressing_matches_direct_conv(emu, case):
     assert rc == 0, emu.emu_last_error().decode()
     assert me.value <= 2e-6 * max(mr.value, 1.0), (me.value, mr.value)  # ~2^-21: hi*hi + lo*hi + hi*lo
     assert sm.value <= 227 * 1024
+
+
+@pytest.mark.parametrize("case", [(8, 16, 1, 2, 0, 1, 1, 4, 70), (32, 16, 1, 2, 0, 1, 1, 4, 70)])
+def test_transposed_conv_with_a_tapless_phase_is_refused(emu, case):
+    """f1s2 (SpatialFullConvolution(1,1,2,2,0,0,1,1)): three of its four sub-pixel phases get no filter tap.  The planner
+    refuses the layer instead of planning an empty phase (tap pairing from 8 channels, the generic plan from 32)."""
+    me, mr, sm, nm = C.c_double(), C.c_double(), C.c_int(), C.c_int()
+    rc = emu.emu_conv_check(*case, 1, C.byref(me), C.byref(mr), C.byref(sm), C.byref(nm))
+    assert rc == 1 and "sub-pixel phase (0,1) without filter taps" in emu.emu_last_error().decode(), emu.emu_last_error()
 
 
 def plan(emu, *case):

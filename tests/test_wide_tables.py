@@ -47,12 +47,12 @@ def test_emulated_style_nblock_jobs_match_direct_conv(emu, case, jobs):
     assert se.value <= 2e-6, se.value  # each block's statistics land in its own channels' slots
 
 
-def _finalize_error(arch, padding_type="reflect-start"):
+def _finalize_error(arch, padding_type="reflect-start", in_dim=7, norm="instance"):
     from fav_b200 import _lib, models_video, synth
 
-    net = models_video.StyleNet(arch, padding_type=padding_type)
+    net = models_video.StyleNet(arch, padding_type=padding_type, in_dim=in_dim, norm=norm)
     try:
-        net.load_state(synth.make_weights(arch, "candy"))
+        net.load_state(synth.make_weights(arch, "candy", in_dim, norm=norm))
     except _lib.FavError as e:
         return e
     return None
