@@ -34,6 +34,8 @@ int launch_temporal_stage_structure(const float *content, const float *prev, con
                                     float *cert_out, const Operand &dst, int R, int H, int W, int r, int border_mode, cudaStream_t st);
 int launch_compute_corners(const float *image, float scale, int Z, int W, int H, float rho, float *corners, float *avg_out,
                            void *workspace, cudaStream_t st);
+int launch_image_scale_bicubic(const float *in, float *out, int C, int Hin, int Win, int Hout, int Wout, cudaStream_t st);
+int check_scale_args(const float *in, const float *out, int C, int Hin, int Win, int Hout, int Wout);
 
 // ---------------------------------------------------------------------------------------------------------
 struct Param {
@@ -107,6 +109,8 @@ struct Plan {
   // allocated on the first such call
   float *structure = nullptr, *structure_avg = nullptr;
   void *corners_ws = nullptr;
+  // -scale_factor (fav_run_image_scaled): the content resampled to this plan's size, allocated on the first such call
+  float *scaled_in = nullptr;
   std::vector<PlanStep> steps;
   std::map<int, int> layer_operand;  // arch token index -> operand holding its output
   // CUDA graphs of the whole per-frame kernel sequence (run_[next_]image), one per destination buffer: a frame is ~40
@@ -961,6 +965,35 @@ int fav_run_image_batch(fav_net_t *net, const float *content, const float *fill,
   }
   FAV_TRY(launch_temporal_input(content, nullptr, nullptr, nullptr, fill, nullptr, pl->in7, H, W, 0, true, st, B));
   return run_plan_frame(net, *pl, pl->in7, out_rgb, st);  // deprocess fused into the last epilogue (core.lua:149)
+}
+
+// a-9 with -scale_factor (core.lua:127-130,146-152): image.scale(img, W*sf, H*sf, 'bicubic') -> model_img(pre(.)) ->
+// deprocess -> image.scale(., W, H, 'bicubic').  The network runs at h x w on the (1, h, w) plan, into the plan's own out3,
+// so the plan keeps one cached graph however many destinations the caller cycles through.
+int fav_run_image_scaled(fav_net_t *net, const float *content, int H, int W, double scale_factor, float *out_rgb, void *stream) {
+  if (scale_factor == 1.0) return fav_run_image(net, content, nullptr, H, W, out_rgb, stream);
+  FAV_REQUIRE(net && content && out_rgb, "fav_run_image_scaled: null argument");
+  FAV_REQUIRE(net->finalized, "fav_run_image_scaled: call fav_net_finalize first");
+  // model_img == nil: the reference concatenates the scaled frame with a fill of the unscaled size, and torch.cat fails
+  FAV_REQUIRE(net->in_dim == 3, "fav_run_image_scaled: -scale_factor %g needs a separate image model (3 input channels); the "
+              "video model's input joins the scaled frame with an unscaled fill (fast_artistic_video_core.lua:133-138)", scale_factor);
+  const double hd = H * scale_factor, wd = W * scale_factor;
+  FAV_REQUIRE(std::isfinite(scale_factor) && scale_factor > 0 && hd == std::floor(hd) && wd == std::floor(wd) && hd < 1e9 &&
+                  wd < 1e9,
+              "fav_run_image_scaled: %dx%d at -scale_factor %g is %gx%g; the scaled frame needs integer sides (image.scale, then "
+              "view(1, 3, H*sf, W*sf), fast_artistic_video_core.lua:128-130)", W, H, scale_factor, wd, hd);
+  const int h = (int)hd, w = (int)wd;
+  FAV_TRY(check_scale_args(content, out_rgb, 3, H, W, h, w));
+  Plan *pl;
+  FAV_TRY(build_plan(net, 1, h, w, &pl));  // the frame rules apply at h x w; refusals come before any device work
+  cudaStream_t st = (cudaStream_t)stream;
+  // not pl->in7: fav_run_image's unfused path (FAV_NO_FUSEPACK) writes that one
+  if (!pl->scaled_in) FAV_TRY(alloc_zero(*pl, (void **)&pl->scaled_in, (size_t)3 * h * w * sizeof(float)));
+  FAV_TRY(launch_image_scale_bicubic(content, pl->scaled_in, 3, H, W, h, w, st));
+  FAV_TRY(launch_temporal_input_packed(pl->scaled_in, nullptr, nullptr, nullptr, nullptr, nullptr, pl->ops[0], net->reflect_pad, h, w,
+                                       0, true, st));
+  FAV_TRY(run_plan_frame(net, *pl, nullptr, pl->out3, st));
+  return launch_image_scale_bicubic(pl->out3, out_rgb, 3, h, w, H, W, st);  // unclamped, like the reference's img_out
 }
 
 int fav_run_next_image(fav_net_t *net, const float *content, const float *prev_rgb, const float *flow,

@@ -98,6 +98,8 @@ SIGNATURES = {
     "fav_debug_set_trace": (C.c_int, [_fp, C.c_size_t]),
     "fav_debug_trace_words": (C.c_size_t, []),
     "fav_run_image": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, _fp, _fp]),
+    "fav_run_image_scaled": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, C.c_double, _fp, _fp]),
+    "fav_image_scale_bicubic": (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     "fav_run_next_image": (C.c_int, [C.c_void_p, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]),
     "fav_run_next_image_flows": (C.c_int, [C.c_void_p, _fp, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp, _fp]),
     "fav_net_forward_batch": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]),

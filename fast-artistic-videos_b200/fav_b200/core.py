@@ -105,8 +105,7 @@ def run_fast_neural_video(opt, func_load_image, func_load_cert, func_eval, func_
     dev = torch.device("cuda", int(_opt(opt, "gpu", 0)) if int(_opt(opt, "gpu", 0)) >= 0 else 0)
     torch.cuda.set_device(dev)
     evaluate = bool(_opt(opt, "evaluate", False))  # :76-98,214-239 -- see the evaluation block at the end of the loop
-    if float(_opt(opt, "scale_factor", 1)) != 1:
-        raise _lib.FavError(_lib.FAV_ERR_UNSUPPORTED, "-scale_factor != 1 (bicubic image.scale) is not on the GPU path")
+    scale_factor = float(_opt(opt, "scale_factor", 1))
     model = model_vid if model_vid is not None else load_model(_opt(opt, "model_vid"), _opt(opt, "arch", synth.DEFAULT_ARCH))
     # get_model (core.lua:59-69): 'self' -> model_img = nil, the video model also stylizes single images
     model_img = model_img if model_img is not None else (
@@ -127,8 +126,11 @@ def run_fast_neural_video(opt, func_load_image, func_load_cert, func_eval, func_
     def run_image(img):  # core.lua:121-158
         t1 = time.perf_counter()
         H, W = img.shape[-2:]
-        if model_img is not None:  # core.lua:146: model_img:forward(img_pre)
-            out = model_img.run_image(img.to(dev))
+        if model_img is not None:  # core.lua:146: model_img:forward(img_pre), between the two image.scale calls of :127-152
+            out = model_img.run_image(img.to(dev), scale_factor=scale_factor)
+        elif scale_factor != 1:  # core.lua:135: the fill has the unscaled size, so torch.cat fails
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, f"-scale_factor {scale_factor} needs -model_img: the video model's input "
+                                "would join the scaled frame with an unscaled fill (fast_artistic_video_core.lua:133-138)")
         else:
             out = model.run_image(img.to(dev), generate_fill(H, W, torch.zeros((1, H, W), device=dev)))
         print("Elapsed time for stylizing frame independently:%f" % (time.perf_counter() - t1))

@@ -103,13 +103,21 @@ class StyleNet:
         return out
 
     # -- fused frame-level ops (fast_artistic_video_core.lua:121-180) ------------------------------------
-    def run_image(self, img: torch.Tensor, fill: torch.Tensor = None) -> torch.Tensor:
-        """img [3,H,W], or [B,3,H,W] for a batch (fill then [B,3,H,W] too)."""
+    def run_image(self, img: torch.Tensor, fill: torch.Tensor = None, scale_factor: float = 1.0) -> torch.Tensor:
+        """img [3,H,W], or [B,3,H,W] for a batch (fill then [B,3,H,W] too).  scale_factor != 1 (-scale_factor, core.lua:127-152):
+        one image [3,H,W] through an image model (in_dim 3), stylized at (H*sf) x (W*sf) between two bicubic image.scale
+        calls (fav_run_image_scaled); fill is then unused, as it is for every image model."""
         x = img.contiguous()
         assert x.dim() in (3, 4) and x.size(-3) == 3 and x.dtype == torch.float32
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
-        if x.dim() == 3:
+        if float(scale_factor) != 1:
+            if x.dim() != 3:
+                raise _lib.FavError(_lib.FAV_ERR_INVALID, f"run_image with scale_factor {scale_factor}: one image [3,H,W], "
+                                    f"got {list(x.shape)}")
+            _lib.check(_lib.lib.fav_run_image_scaled(self._h, _lib.dptr(x), H, W, C.c_double(float(scale_factor)),
+                                                     _lib.dptr(out), _lib.stream_ptr()))
+        elif x.dim() == 3:
             _lib.check(_lib.lib.fav_run_image(self._h, _lib.dptr(x), _lib.dptr(fill), H, W, _lib.dptr(out),
                                               _lib.stream_ptr()))
         else:

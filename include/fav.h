@@ -273,12 +273,27 @@ FAV_API size_t fav_debug_trace_words(void);
 /* a-9  run_image                               fast_artistic_video_core.lua:121-158
  * content [3,H,W] RGB [0,1] -> out_rgb [3,H,W] = deprocess(model(...))[1].  A net created with in_dim = 7 is the video model
  * fed cat(pre(img), fill, zeros) (model_img == nil, :133-138); in_dim = 3 is a separate image model fed pre(img) (:146, fill
- * is ignored).  -scale_factor != 1 (bicubic image.scale of the un-vendored `image` rock, :127-129,150-152) is not built.
+ * is ignored).  -scale_factor != 1 is fav_run_image_scaled below.
  * fav_run_image / fav_run_next_image enqueue the fused input kernel plus ONE CUDA-graph launch of the network (captured on
  * the second call for each distinct out_rgb pointer, 8 graphs cached per frame size): ping-pong a few output buffers.
  * One stream at a time per net (it owns the activation buffers), like model:forward in the reference. */
 FAV_API int fav_run_image(fav_net_t *net, const float *content, const float *fill, int H, int W,
                           float *out_rgb, void *stream);
+/* a-9 with -scale_factor                        fast_artistic_video_core.lua:121-158 (fast_artistic_video.lua:42)
+ * content [3,H,W] -> out_rgb [3,H,W] = image.scale(deprocess(model_img(pre(image.scale(content, W*sf, H*sf, 'bicubic')))),
+ * W, H, 'bicubic') (:127-130,146-152), unclamped (the reference keeps it as last_frame_stylized, fast_artistic_video.lua:169).
+ * scale_factor == 1 is exactly fav_run_image(net, content, NULL, H, W, out_rgb, stream).  Otherwise the net must be an image
+ * model (in_dim 3): the video model's input would join the scaled frame with an unscaled fill, which the reference's torch.cat
+ * refuses (:133-138).  h = H*sf and w = W*sf (in double) must be integers, and h x w must satisfy the frame rules of every
+ * run_* call (multiples of 4, at least 16, larger than the reflection padding).  Every refusal is FAV_ERR_INVALID, before any
+ * device work.  The network runs at h x w as ONE cached graph launch, between the two fav_image_scale_bicubic kernels. */
+FAV_API int fav_run_image_scaled(fav_net_t *net, const float *content, int H, int W, double scale_factor, float *out_rgb,
+                                 void *stream);
+/* image.scale(src, Wout, Hout, 'bicubic') of the `image` rock (fast_artistic_video_core.lua:128,151; the rock is not vendored,
+ * DESIGN.md 8 states the reading): in [C,Hin,Win] -> out [C,Hout,Wout], planar fp32.  Separable Catmull-Rom on an
+ * align-corners grid, linearly extrapolated borders, no prefilter, no clamping; a side of equal size is copied.  Sizes 2 to
+ * 65535 (FAV_ERR_INVALID otherwise, a side of 1 included). */
+FAV_API int fav_image_scale_bicubic(const float *in, float *out, int C, int Hin, int Win, int Hout, int Wout, void *stream);
 /* a-8  run_next_image                           fast_artistic_video_core.lua:161-180
  * (+ func_make_last_frame_warped, fast_artistic_video.lua:153-158: the warp of prev_rgb by flow) */
 FAV_API int fav_run_next_image(fav_net_t *net, const float *content, const float *prev_rgb,
