@@ -147,6 +147,27 @@ __host__ __device__ inline bool opnd_epi_addr(const ConvJob &j, int tile, int t,
   return opnd_epi_addr(j, tile_at(j, tile, batch), t, i, h, dst4, skip4);
 }
 
+// Norm-on-load addressing, shared by the producer warps of conv_tc_kernel and their CPU emulator (tests/emu/nl_geom_emu.cu).
+// The producer stages, for every patch pixel, the value the bulk copies would read from the operand that in_apply writes:
+// patch row ri of group g is raw row nl_raw_row, pixel p of a (patch row, channel block) slab is raw column nl_raw_col, and
+// a pixel outside [0, nl_H) x [0, nl_W) is zero (the operand's zero border).  One segment: storage column seg_src16[0] + x0 + p.
+// Two segments (stride-2 consumers, parity-split operand [Cb][2][Ws2]): segment s is parity plane s, so its pixel
+// p - seg_dst16[s] is storage column 2 (x0 + p - seg_dst16[s]) + s.
+__host__ __device__ inline int nl_raw_row(const ConvJob &j, int y, int g, int ri) { return j.row_mul * y + j.grp_row[g][ri] - j.nl_padT; }
+__host__ __device__ inline int nl_raw_col(const ConvJob &j, int x0, int p) {
+  if (j.nseg == 1) return j.seg_src16[0] + x0 + p - j.nl_padL;
+  const int s = p >= j.seg_dst16[1] ? 1 : 0;
+  return 2 * (x0 + p - j.seg_dst16[s]) + s - j.nl_padL;
+}
+// the patch layouts the norm-on-load producer can fill (nl_raw_col): every pixel of a slab comes from one storage row, in one
+// segment, or in the two parity segments of a stride-2 consumer
+__host__ __device__ inline bool nl_geometry_ok(const ConvJob &j) {
+  if (j.rf_R || j.pf || j.opnd || j.mt != 1) return false;
+  if (j.nseg == 1) return j.seg_dst16[0] == 0 && j.seg_len16[0] == j.pslab16;
+  return j.nseg == 2 && j.seg_src16[0] == 0 && j.seg_dst16[0] == 0 && j.seg_dst16[1] == j.seg_len16[0] &&
+         j.seg_len16[0] + j.seg_len16[1] == j.pslab16 && j.seg_src16[1] == j.a_slab16 / 2;
+}
+
 // CUDA-core comparator job (debug / bring-up path; same inputs and outputs as ConvJob)
 struct SimtJob {
   Operand in;

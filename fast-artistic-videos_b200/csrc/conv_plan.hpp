@@ -399,6 +399,18 @@ static inline void set_opnd_epilogue(ConvJob &j, int b, const float *scale, cons
   j.epi_skip = skip ? 1 : 0; j.epi_skip_op = skip ? *skip : Operand(); j.epi_shave = skip ? shave : 0;
   j.raw = nullptr; j.stats = nullptr;
 }
+// norm-on-load (conv_tc.cu): job j reads `raw`, the raw output of the previous convolution, and applies its InstanceNorm
+// (+ReLU) and the fp16 hi / lo split while it stages the patch, instead of reading `in`, the operand in_apply would write from
+// it (nl_raw_row / nl_raw_col, conv.cuh).  sums: raw's fused statistics, sums_img doubles apart per image.
+static inline void set_norm_on_load(ConvJob &j, const RawTensor &raw, const Operand &in, int relu, const double *sums,
+                                    int64_t sums_img, const float *gamma, const float *beta) {
+  j.nl = 1;
+  j.nl_raw = reinterpret_cast<const float4 *>(raw.p); j.nl_Cq = raw.Cq; j.nl_Wp = raw.Wp; j.nl_H = raw.H; j.nl_W = raw.W;
+  j.nl_padT = in.padT; j.nl_padL = in.padL; j.nl_relu = relu; j.nl_C = raw.C;
+  j.nl_sums = sums; j.nl_gamma = gamma; j.nl_beta = beta;
+  j.nl_raw_img4 = raw.img / 4; j.nl_sums_img = sums_img;
+  j.nl_inv_count = 1.0 / ((double)raw.H * raw.W); j.nl_eps = 1e-5;  // InstanceNormalization.lua:21
+}
 // a batch of nimg images of one size (conv.cuh tile_at): per-image strides of the job's raw output (floats), final frame (floats)
 // and fused statistics (doubles); the A operand's and the operand epilogue's come with their Operands (Operand::img16)
 static inline void set_conv_batch(ConvJob &j, int nimg, int64_t raw_img, int64_t out3_img, int64_t stats_img) {

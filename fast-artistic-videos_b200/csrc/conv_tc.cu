@@ -21,7 +21,7 @@
 //               (or x-fold reduction + tanh/deprocess for the last layer)
 //   warp  8     B producer (bulk copies of weight chunks)
 //   warp  9     A producer (bulk copies of the patch, all lanes issue)
-//   warps 9-12  norm-on-load jobs: patch producers (raw fp32 -> InstanceNorm + ReLU -> fp16 hi/lo staged for the MMA,
+//   warps 9-15  norm-on-load jobs: patch producers (raw fp32 -> InstanceNorm + ReLU -> fp16 hi/lo staged for the MMA,
 //               replacing a separate in_apply pass)
 // Plans per layer family (conv_plan.hpp): generic, stride-2 parity split, tap pairing (Cin = 8), x-fold.
 // Pipelines: A stages and weight slots with full/empty mbarriers; each consumer warpgroup releases a slot once its
@@ -38,7 +38,9 @@ constexpr int kMaxA = 4;  // patch stages
 constexpr int kMaxB = 16;  // weight slots (ring or resident)
 constexpr int kConsumerThreads = 256;  // warps 0-7
 constexpr int kBWarp = 8, kAWarp = 9;
-constexpr int kNlWarps = 4;            // norm-on-load producers: warps 9..12
+// norm-on-load producers: warps 9..15.  Seven warps fill the 512 threads one CTA can have at the 128 registers the consumers
+// need; the producers are latency bound (one L2 round trip per unit of work), so each warp more adds loads in flight
+constexpr int kNlWarps = 7;
 constexpr int kThreads = kConsumerThreads + 32 * (1 + kNlWarps);  // launched with 320 threads when nl == 0
 constexpr int kNlPx = 5;        // pixels in flight per lane (5 x 32 >= the 130-pixel patch row)
 constexpr int kNlMaxC = 256;
@@ -312,7 +314,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) exch[256 + i] = 0.f;
   // norm-on-load: mean / gamma*rstd / beta per input channel from the producer conv's fused statistics (same arithmetic
   // as in_apply_kernel: biased variance, eps inside the sqrt, InstanceNormalization.lua:39-50)
-  float *nl_tab = exch + (256 + 8 * 2 * 128);
+  // (after the x-fold exchange buffer, or after the statistics slots: tc_fixed_smem)
+  float *nl_tab = exch + (job.xfold_kw ? kTileM * kExchPitch : 256 + 8 * 2 * 128);
   const int total = (BATCH ? job.nimg : 1) * job.ntiles;
   int nl_b = BATCH ? (int)blockIdx.x / job.ntiles : 0;  // image whose statistics nl_tab holds
   if (job.nl) nl_build_table(job, nl_tab, nl_b, threadIdx.x, blockDim.x);
@@ -325,41 +328,42 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     tc_consume<NT, OPND, BATCH>(job, a_base, b_base, sh, exch);
   } else if (job.nl && warp >= kAWarp) {
     // ===== norm-on-load patch producers: raw fp32 -> InstanceNorm (+ReLU) -> fp16 hi/lo -> MMA-ready stage =====
-    // A warp owns whole (patch row, channel block) slabs: lanes run along x (coalesced 512-byte loads), up to
-    // kNlPx float4 pairs in flight per lane, no per-pixel index arithmetic.
+    // The warps take turns over units of 32 kNlPx pixels of one (patch row, channel block) slab: lanes run along the slab,
+    // kNlPx float4 pairs in flight per lane.  Units rather than whole slabs keep the warps evenly loaded when a slab is longer
+    // than one unit (the 257 pixels of a stride-2 consumer).
     const int pw = warp - kAWarp;
-    const int pslab = job.pslab16, nslabs = job.nrows * job.CbG;
+    const int pslab = job.pslab16, nck = (pslab + 32 * kNlPx - 1) / (32 * kNlPx), nunits = job.nrows * job.CbG * nck;
     uint32_t s = 0, ph = 0;
     for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
       const TileAt at = tile_at(job, tile, BATCH);
-      const int y = at.y;
-      const int xb = job.seg_src16[0] + at.x0 - job.nl_padL;  // raw column of patch pixel 0
+      const int y = at.y, x0 = at.x0;
       if (at.b != nl_b) {
-        // the next image: its table replaces the current one once all four producer warps are done with the previous tile
+        // the next image: its table replaces the current one once all producer warps are done with the previous tile
         nl_b = at.b;
-        asm volatile("bar.sync 2, 128;" ::: "memory");
+        asm volatile("bar.sync 2, %0;" ::"r"(32 * kNlWarps) : "memory");
         nl_build_table(job, nl_tab, nl_b, threadIdx.x - kAWarp * 32, 32 * kNlWarps);
-        asm volatile("bar.sync 2, 128;" ::: "memory");
+        asm volatile("bar.sync 2, %0;" ::"r"(32 * kNlWarps) : "memory");
       }
       const float4 *nl_raw = job.nl_raw + at.nl_raw4;
       for (int g = 0; g < ngroups; ++g) {
         mbar_wait(&sh->a_empty[s], ph ^ 1);
         uint8_t *stage = a_base + s * 2 * a_stage_bytes;
-        for (int rc = pw; rc < nslabs; rc += kNlWarps) {
+        for (int u = pw; u < nunits; u += kNlWarps) {
+          const int rc = u / nck, pb = (u - rc * nck) * 32 * kNlPx;
           const int ri = rc / job.CbG, cbi = rc - ri * job.CbG;
-          const int ry = job.row_mul * y + job.grp_row[g][ri] - job.nl_padT, cb = job.grp_cb0[g] + cbi;
+          const int ry = nl_raw_row(job, y, g, ri), cb = job.grp_cb0[g] + cbi;
           const bool row_ok = ry >= 0 && ry < job.nl_H;
           const float4 *rp = nl_raw + ((int64_t)(row_ok ? ry : 0) * job.nl_Cq + 2 * cb) * job.nl_Wp;
           float tm[8], ts[8], tb[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) { tm[i] = nl_tab[cb * 8 + i]; ts[i] = nl_tab[kNlMaxC + cb * 8 + i]; tb[i] = nl_tab[2 * kNlMaxC + cb * 8 + i]; }
           uint8_t *drow = stage + (uint32_t)(rc * pslab) * 16u;
-          for (int pb = 0; pb < pslab; pb += 32 * kNlPx) {
+          {
             float4 va[kNlPx], vb[kNlPx];
             uint32_t okm = 0;
 #pragma unroll
             for (int k = 0; k < kNlPx; ++k) {
-              const int p = pb + k * 32 + lane, x = xb + p;
+              const int p = pb + k * 32 + lane, x = nl_raw_col(job, x0, p);
               const bool ok = row_ok && p < pslab && x >= 0 && x < job.nl_W;
               // unconditional loads from a clamped (always valid) address: all 2 * kNlPx requests are issued back to back
               const int xc = x < 0 ? 0 : (x < job.nl_Wp ? x : job.nl_Wp - 1);

@@ -80,11 +80,12 @@ struct PlanStep {
   int shave = 2;
   RawTensor raw;
   std::vector<ConvJob> tc;
+  std::vector<ConvJob> tc_plain;  // kind 0 normalising on load: the same jobs reading the in_apply'd operand (replay_unfused)
   std::vector<SimtJob> simt;
   int stats_off = 0;
   int raw_sel = 0;       // raw.p is Plan::raw_buf (0) or raw_buf2 (1)
   int layer_index = -1;  // arch token index whose output this step completes (for fav_net_layer_output)
-  bool fused_nl = false; // kind 1: the tcgen05 consumer normalises on load (conv_tc.cu), this pass is skipped
+  bool fused_nl = false; // kind 1: the tensor-core consumer normalises on load (conv_tc.cu), this pass is skipped
 };
 
 // a batch: B frames of one size run through one plan, every kernel covering all B images in one launch (conv.cuh tile_at);
@@ -385,6 +386,36 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
   return FAV_OK;
 }
 
+// Fold the InstanceNorm (+ReLU) pass just planned (the last step) into the patch producers of conv step cs, its only reader:
+// the pass then never runs and cs normalises the raw tensor while it loads it (conv_tc.cu norm-on-load).  Not for a pass that
+// adds a skip or whose operand a later step reads as a skip (src_is_skip: the first conv of a residual block), and only when
+// every job of cs has a patch layout the producers can fill (nl_geometry_ok) and still fits shared memory.  Each N block of a
+// wide conv normalises the whole patch itself; the per-channel tables hold at most 256 channels (conv_tc.cu kNlMaxC).  The
+// unfused jobs stay in cs.tc_plain for fav_net_layer_output (run_plan's replay).  FAV_NO_NL switches every fusion off.
+// The x-fold final conv stays unfused although the producers could fill its patch: it normalises every raw pixel once per
+// filter row and ran slower fused than the pass it would remove (DESIGN.md 4.1, H100 at 720p: 0.485 ms against 0.271 ms
+// + a 0.086 ms pass).
+static void fuse_norm_on_load(fav_net *net, Plan &pl, PlanStep &cs, bool src_is_skip) {
+  if (net->bn || src_is_skip || pl.steps.empty() || getenv("FAV_NO_NL")) return;
+  PlanStep &ap = pl.steps.back();
+  if (ap.kind != 1 || ap.skip >= 0 || ap.dst != cs.src) return;
+  const InDef &n = net->inorms[ap.inorm];
+  if (n.C > 256) return;
+  std::vector<ConvJob> fused;
+  for (const ConvJob &j : cs.tc) {
+    if (!nl_geometry_ok(j) || j.xfold_kw) return;
+    ConvJob t = j;
+    set_norm_on_load(t, ap.raw, pl.ops[cs.src], ap.relu, pl.stats + ap.stats_off, pl.stats_img, n.d_gamma, n.d_beta);
+    conv_tc_choose_slots(t);
+    if (conv_tc_smem_bytes(t) > 227 * 1024 || !(t.b_resident || t.b_slots >= 2)) return;
+    fused.push_back(t);
+  }
+  if (fused.empty()) return;
+  cs.tc_plain = std::move(cs.tc);
+  cs.tc = std::move(fused);
+  ap.fused_nl = true;
+}
+
 static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
   if (B < 1 || B > kMaxBatch) {
     set_error("batch of %d frames: 1 to %d frames per call", B, kMaxBatch);
@@ -481,6 +512,7 @@ static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
       const bool last = op.last && i == n - 1;
       if (last) {
         FAV_TRY(build_conv_jobs(net, *pl, cs, c, true, nullptr, nullptr));
+        fuse_norm_on_load(net, *pl, cs, false);
         cs.layer_index = (int)oi;
         pl->steps.push_back(std::move(cs));
         break;
@@ -507,33 +539,7 @@ static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
       // which then only runs after the CUDA-core comparator
       FAV_TRY(build_conv_jobs(net, *pl, cs, c, false, nullptr, net->bn ? nullptr : pl->stats + ns.stats_off,
                               net->bn ? &ns : nullptr));
-      // second conv of a residual block: fold the preceding InstanceNorm + ReLU pass into its patch producers.  Each N block
-      // of a wide conv normalises the whole patch on load itself (the A-side work is repeated per block); the per-channel
-      // tables hold at most 256 channels (conv_tc.cu kNlMaxC), wider blocks keep the separate in_apply pass.
-      if (!net->bn && op.kind == 1 && i == 1 && !pl->steps.empty() && pl->steps.back().kind == 1 && !getenv("FAV_NO_NL")) {
-        PlanStep &ap = pl->steps.back();
-        const InDef &n = net->inorms[ap.inorm];
-        const Operand &in = pl->ops[cs.src];
-        bool ok = ap.skip < 0 && n.C <= 256;
-        std::vector<ConvJob> fused;
-        for (size_t k = 0; ok && k < cs.tc.size(); ++k) {
-          const ConvJob &j = cs.tc[k];
-          ok = !j.rf_R && !j.pf && !j.xfold_kw && j.nseg == 1 && j.seg_dst16[0] == 0 && j.seg_len16[0] == j.pslab16 && j.row_mul == 1;
-          if (ok) {
-            ConvJob t = j;
-            t.nl = 1;
-            t.nl_raw = reinterpret_cast<const float4 *>(ap.raw.p); t.nl_Cq = ap.raw.Cq; t.nl_Wp = ap.raw.Wp;
-            t.nl_H = ap.raw.H; t.nl_W = ap.raw.W; t.nl_padT = in.padT; t.nl_padL = in.padL; t.nl_relu = ap.relu; t.nl_C = n.C;
-            t.nl_sums = pl->stats + ap.stats_off; t.nl_gamma = n.d_gamma; t.nl_beta = n.d_beta;
-            t.nl_raw_img4 = ap.raw.img / 4; t.nl_sums_img = pl->stats_img;
-            t.nl_inv_count = 1.0 / ((double)ap.raw.H * ap.raw.W); t.nl_eps = 1e-5;
-            conv_tc_choose_slots(t);
-            ok = conv_tc_smem_bytes(t) <= 227 * 1024 && (t.b_resident || t.b_slots >= 2);
-            fused.push_back(t);
-          }
-        }
-        if (ok && !fused.empty()) { cs.tc = std::move(fused); ap.fused_nl = true; }
-      }
+      fuse_norm_on_load(net, *pl, cs, op.kind == 1 && i == 0 && op.skip);
       pl->steps.push_back(std::move(cs));
       cur = ns.dst;
       if (i == n - 1) { ns.layer_index = (int)oi; pl->layer_operand[(int)oi] = cur; }
@@ -568,8 +574,10 @@ static int ensure_raw(Plan &pl) {
 }
 
 // in7 == nullptr: the caller has already written the first operand (fused temporal input, run_plan_frame)
+// last >= 0: steps 0..last only.  unfused: the passes the plan folds into their consumers run, and the consumers read their
+// operands (replay_unfused)
 static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int final_mode, cudaStream_t st,
-                    std::vector<ProfRec> *prof = nullptr) {
+                    std::vector<ProfRec> *prof = nullptr, int last = -1, bool unfused = false) {
   auto begin = [&](int kind, double work, const std::string &name) -> int {
     if (!prof) return FAV_OK;
     ProfRec r;
@@ -592,7 +600,8 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
     FAV_TRY(launch_pack_input(in7, net->in_dim, pl.H, pl.W, net->reflect_pad, pl.ops[0], st, pl.B));
     FAV_TRY(end());
   }
-  for (PlanStep &s : pl.steps) {
+  for (size_t si = 0; si < pl.steps.size() && (last < 0 || (int)si <= last); ++si) {
+    PlanStep &s = pl.steps[si];
     if (s.kind == 0) {
       {
         const ConvDef &c = net->convs[s.conv];
@@ -601,7 +610,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
         FAV_TRY(begin(1, 2.0 * c.cin * c.cout * c.k * c.k * px, c.name));
       }
       if (net->conv_impl == 0) {
-        for (ConvJob &j : s.tc) {
+        for (ConvJob &j : (unfused && !s.tc_plain.empty()) ? s.tc_plain : s.tc) {
           if (j.final_mode) { j.final_mode = final_mode; j.out3 = out3; }
           FAV_TRY(launch_conv_tc(j, net->num_sms, st));
         }
@@ -626,7 +635,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
                            n.d_scale, pl.B, pl.stats_img));
       FAV_TRY(end());
     } else {
-      if (s.fused_nl && net->conv_impl == 0) continue;  // the consumer conv normalises while it loads (norm-on-load)
+      if (s.fused_nl && net->conv_impl == 0 && !unfused) continue;  // the consumer conv normalises while it loads (norm-on-load)
       const InDef &n = net->inorms[s.inorm];
       if (net->bn) {  // BatchNorm folded into the conv: its tensor-core epilogue wrote the operand
         if (net->conv_impl == 0) continue;
@@ -938,6 +947,15 @@ int fav_net_layer_output_image(fav_net_t *net, int index, int b, float *out, int
   if (Hl) *Hl = o.H;
   if (Wl) *Wl = o.W;
   if (!out) return FAV_OK;
+  // a pass folded into its consumer (norm-on-load) never wrote this operand: replay the forward up to it with the pass run.
+  // The replay starts from the net's first operand, which the forward leaves intact, so it recomputes the same bits.
+  for (size_t si = 0; si < pl->steps.size(); ++si) {
+    const PlanStep &s = pl->steps[si];
+    if (s.layer_index == index && s.kind == 1 && s.fused_nl && net->conv_impl == 0) {
+      FAV_TRY(run_plan(net, *pl, nullptr, nullptr, 1, (cudaStream_t)stream, nullptr, (int)si, true));
+      break;
+    }
+  }
   return launch_unpack_operand(image_of(o, b), out, (cudaStream_t)stream);
 }
 
