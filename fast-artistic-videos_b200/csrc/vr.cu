@@ -6,6 +6,9 @@
 //       out = base * (1 - mask) + mask * sum_{i<4} warp(rot_i(side_i), map_i) / div
 //       -- the reference runs 4 warp launches, 4 rotations (index copies), 4 divisions, 3 adds, 2 cmuls, 1 add per face;
 //       here the rotation is an index mapping inside the gather and everything is one kernel.
+//   -evaluate gradient metric     evaluate_gradient              fast_artistic_video_vr.lua:344-387
+//       (the six double sums behind gradx / grady / gradmag: face gradients, max-pooled mask gradients and their products
+//        in one pass over a shared-memory tile; the reference runs it on the CPU in double)
 // Arithmetic follows the reference order with round-to-nearest intrinsics (bit-exact vs the oracle composition).
 #include "fav_common.cuh"
 
@@ -100,6 +103,115 @@ __global__ void __launch_bounds__(256) vr_blend_kernel(const __grid_constant__ B
   }
 }
 
+// ---- -evaluate gradient metric (evaluate_gradient, fast_artistic_video_vr.lua:344-387) -----------------------------
+// One CTA per kEvTX x kEvTY tile of the H x W grid; thread t owns column x0 + t and walks the tile's rows.  Everything is in
+// double from the fp32 inputs, as the reference computes after :double():
+//   gx = max_c |f[c][y][x+2] - f[c][y][x]|  on [H, W-2]      gy = max_c |f[c][y+2][x] - f[c][y][x]|  on [H-2, W]
+//   MX = 3x3 max-pool (stride 1, padding cells ignored) of |m[y][x+2] - m[y][x]| on [H, W-2], MY likewise on [H-2, W].
+// The pool is separable: each row's 3-wide horizontal maximum is formed once and the vertical maximum slides over three of
+// them in registers.  Out-of-domain cells enter as 0, which leaves the maximum of non-negative values unchanged.
+// Sums: per thread in row order, per CTA by a fixed tree, then vr_eval_finish_kernel adds the CTA partials in tile order.
+constexpr int kEvTX = 128, kEvTY = 16;
+
+__global__ void __launch_bounds__(kEvTX) vr_eval_gradient_kernel(const float *__restrict__ face, const float *__restrict__ mask,
+                                                                 int H, int W, double *__restrict__ part) {
+  __shared__ float sf[3][kEvTY + 2][kEvTX + 2];  // face rows y0 .. y0+TY+1, columns x0 .. x0+TX+1
+  __shared__ float sm[kEvTY + 4][kEvTX + 4];     // mask rows y0-1 .. y0+TY+2, columns x0-1 .. x0+TX+2
+  __shared__ double red[kEvTX];
+  const int x0 = blockIdx.x * kEvTX, y0 = blockIdx.y * kEvTY, t = threadIdx.x;
+  const int64_t HW = (int64_t)H * W;
+  for (int i = t; i < 3 * (kEvTY + 2) * (kEvTX + 2); i += kEvTX) {
+    const int c = i / ((kEvTY + 2) * (kEvTX + 2)), r = i / (kEvTX + 2) % (kEvTY + 2), q = i % (kEvTX + 2);
+    const int gy = y0 + r, gx = x0 + q;
+    sf[c][r][q] = (gy < H && gx < W) ? __ldg(face + c * HW + (int64_t)gy * W + gx) : 0.f;
+  }
+  for (int i = t; i < (kEvTY + 4) * (kEvTX + 4); i += kEvTX) {
+    const int r = i / (kEvTX + 4), q = i % (kEvTX + 4);
+    const int gy = y0 - 1 + r, gx = x0 - 1 + q;
+    sm[r][q] = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? __ldg(mask + (int64_t)gy * W + gx) : 0.f;
+  }
+  __syncthreads();
+
+  const int x = x0 + t;
+  // horizontal 3-maxima of |dm_x| (domain [H, W-2]) and |dm_y| (domain [H-2, W]) of global row gy, for this column
+  auto hmax_x = [&](int gy) {
+    double v = 0.0;
+    if (gy < 0 || gy >= H) return v;
+    const float *row = &sm[gy - y0 + 1][t + 1];  // row[d] = m[gy][x + d]
+#pragma unroll
+    for (int d = -1; d <= 1; ++d)
+      if (x + d >= 0 && x + d < W - 2) v = fmax(v, fabs((double)row[d + 2] - (double)row[d]));
+    return v;
+  };
+  auto hmax_y = [&](int gy) {
+    double v = 0.0;
+    if (gy < 0 || gy >= H - 2) return v;
+    const float *r0 = &sm[gy - y0 + 1][t + 1], *r2 = &sm[gy - y0 + 3][t + 1];
+#pragma unroll
+    for (int d = -1; d <= 1; ++d)
+      if (x + d >= 0 && x + d < W) v = fmax(v, fabs((double)r2[d] - (double)r0[d]));
+    return v;
+  };
+  double s_gx = 0.0, s_gy = 0.0, s_mx = 0.0, s_my = 0.0, s_gxm = 0.0, s_gym = 0.0;
+  if (x < W) {
+    double ax = hmax_x(y0 - 1), bx = hmax_x(y0), ay = hmax_y(y0 - 1), by = hmax_y(y0);
+    const int ye = min(kEvTY, H - y0);
+    for (int r = 0; r < ye; ++r) {
+      const int y = y0 + r;
+      const double cx = hmax_x(y + 1), cy = hmax_y(y + 1);
+      if (x < W - 2) {
+        const double mx = fmax(fmax(ax, bx), cx);
+        double g = 0.0;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) g = fmax(g, fabs((double)sf[c][r][t + 2] - (double)sf[c][r][t]));
+        s_gx += g;
+        s_mx += mx;
+        s_gxm += __dmul_rn(g, mx);  // cmul, then sum: the product is rounded on its own
+      }
+      if (y < H - 2) {
+        const double my = fmax(fmax(ay, by), cy);
+        double g = 0.0;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) g = fmax(g, fabs((double)sf[c][r + 2][t] - (double)sf[c][r][t]));
+        s_gy += g;
+        s_my += my;
+        s_gym += __dmul_rn(g, my);
+      }
+      ax = bx; bx = cx; ay = by; by = cy;
+    }
+  }
+  const double v[6] = {s_gx, s_gy, s_mx, s_my, s_gxm, s_gym};
+  const int64_t nt = (int64_t)gridDim.x * gridDim.y, b = (int64_t)blockIdx.y * gridDim.x + blockIdx.x;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) {
+    red[t] = v[k];
+    __syncthreads();
+#pragma unroll
+    for (int s = kEvTX / 2; s > 0; s >>= 1) {
+      if (t < s) red[t] += red[t + s];
+      __syncthreads();
+    }
+    if (t == 0) part[k * nt + b] = red[0];
+    __syncthreads();
+  }
+}
+
+// sums[k] = sum over tiles, in tile order, of part[k][tile]: CTA k adds row k
+__global__ void __launch_bounds__(256) vr_eval_finish_kernel(const double *__restrict__ part, int64_t nt, double *__restrict__ sums) {
+  __shared__ double red[256];
+  const int t = threadIdx.x;
+  double s = 0.0;
+  for (int64_t i = t; i < nt; i += 256) s += part[blockIdx.x * nt + i];
+  red[t] = s;
+  __syncthreads();
+#pragma unroll
+  for (int k = 128; k > 0; k >>= 1) {
+    if (t < k) red[t] += red[t + k];
+    __syncthreads();
+  }
+  if (t == 0) sums[blockIdx.x] = red[0];
+}
+
 }  // namespace fav
 
 using namespace fav;
@@ -133,5 +245,26 @@ int fav_vr_blend_sides(const float *base, const float *const sides[4], const flo
   dim3 block(32, 8), grid(ceil_div(S, 32), ceil_div(S, 8));
   vr_blend_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(a);
   return post_launch("vr_blend_sides");
+}
+
+int fav_vr_eval_gradient(const float *face, const float *mask, int H, int W, double *sums_dev, void *stream) {
+  FAV_REQUIRE(face && mask && sums_dev, "vr_eval_gradient: null argument");
+  FAV_REQUIRE(H >= 3 && W >= 3, "vr_eval_gradient: face %dx%d, need H, W >= 3", H, W);
+  FAV_REQUIRE(ceil_div(H, kEvTY) <= 65535, "vr_eval_gradient: H %d too large", H);
+  FAV_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid(ceil_div(W, kEvTX), ceil_div(H, kEvTY));
+  const int64_t nt = (int64_t)grid.x * grid.y;
+  // the CTA partials live on the stream's own pool allocation, so concurrent calls on different streams never share them
+  double *part = nullptr;
+  FAV_TRY(check_cuda(cudaMallocAsync((void **)&part, (size_t)nt * 6 * sizeof(double), st), "vr_eval_gradient: partials"));
+  vr_eval_gradient_kernel<<<grid, kEvTX, 0, st>>>(face, mask, H, W, part);
+  int rc = post_launch("vr_eval_gradient");
+  if (rc == FAV_OK) {
+    vr_eval_finish_kernel<<<6, 256, 0, st>>>(part, nt, sums_dev);
+    rc = post_launch("vr_eval_gradient finish");
+  }
+  const int rf = check_cuda(cudaFreeAsync(part, st), "vr_eval_gradient: free partials");
+  return rc != FAV_OK ? rc : rf;
 }
 }

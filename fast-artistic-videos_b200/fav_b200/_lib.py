@@ -64,6 +64,7 @@ SIGNATURES = {
     "fav_median_filter": (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     "fav_vr_blend_sides": (C.c_int, [_fp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int), _fp, _fp, _fp, _fp,
                                      C.c_int, _fp]),
+    "fav_vr_eval_gradient": (C.c_int, [_fp, _fp, C.c_int, C.c_int, _fp, _fp]),
     "fav_flo_read_header": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "fav_flo_read": (C.c_int, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_int]),
     "fav_pnm_read_header": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),

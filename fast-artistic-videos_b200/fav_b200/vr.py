@@ -6,8 +6,18 @@ Every warp goes through nn.BilinearSamplerBDHW's replacement (fav_bilinear_sampl
 re-blend is ONE fused kernel per face (fav_vr_blend_sides: 4 rotated gathers + combineSides + blend) instead of
 4 warps + 4 rotations + 10 elementwise passes; the median runs on the GPU.  Mask algebra that happens once per stream
 (init, :164-198) or on single-channel masks uses torch elementwise ops as plumbing.
--evaluate is out of scope (needs VGG-16 weights).  -invert_occlusions / -fix_occlusions are parsed and ignored, exactly as
-in the reference (its VR func_load_cert, :204-237, never reads them)."""
+-invert_occlusions / -fix_occlusions are parsed and ignored, exactly as in the reference (its VR func_load_cert, :204-237,
+never reads them).
+
+-evaluate (func_eval, :312-452) scores every face after it is saved: the gradient metric along the cut edges
+(evaluate_gradient: six double sums from ONE kernel, fav_vr_eval_gradient), the seam MSE of the trimmed faces (evaluate_edge /
+evaluate_edge_top, double-precision torch plumbing on O(S) elements), the content and style losses through the loss network
+(core.make_evaluate_image; nan without one) and the temporal MSE (fav_temporal_mse).  The reference's quirks are kept: mode 3
+compares the same face pair twice, evaluate_edge_top reads only its second argument (its 'top' term is 0), face 4's temporal
+term sees prev_last_segments already replaced by this frame's re-blend, and -fix_occlusions_eval uses the VR script's own
+per-pixel rule (:117-128).  The reference reads opt.reliable_map_min_filter without declaring it (:408-424); here it is an
+option with train_video.lua's default 7.  Unequal overlaps are refused with -evaluate: the mode-4 MSE would compare slices of
+different lengths (DESIGN.md section 8)."""
 from __future__ import annotations
 
 import argparse
@@ -47,6 +57,17 @@ def getFormatedFlowFileName(pattern, fromIndex, toIndex, modeIdx):  # :108-115
     return s % modeIdx
 
 
+def gradient_ratios(sums, H, W):
+    """gradx, grady, gradmag of evaluate_gradient (:375-386) from fav_vr_eval_gradient's six sums
+    (sum gx, sum gy, sum MX, sum MY, sum gx*MX, sum gy*MY), with IEEE double semantics as Lua: 0/0 is nan, x/0 is inf."""
+    Sgx, Sgy, Smx, Smy, Sgxm, Sgym = (np.float64(v) for v in sums)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        gradx = (Sgxm / Smx) / (Sgx / np.float64(H * (W - 2)))
+        grady = (Sgym / Smy) / (Sgy / np.float64((H - 2) * W))
+        gradmag = (gradx * Smx + grady * Smy) / (Smx + Smy)
+    return float(gradx), float(grady), float(gradmag)
+
+
 def build_parser():
     p = argparse.ArgumentParser(prefix_chars="-")
     a = p.add_argument
@@ -62,6 +83,16 @@ def build_parser():
     a("-out_equi", action="store_true"); a("-out_cubemap", action="store_true"); a("-median_filter", type=int, default=3)
     a("-gpu", type=int, default=0); a("-backend", default="cuda"); a("-use_cudnn", type=int, default=1)
     a("-cudnn_benchmark", type=int, default=0); a("-evaluate", action="store_true")
+    # evaluation (:59-74); -loss_network names the .t7 loss network (without one, and no models/vgg16.t7, the perceptual rows are nan)
+    a("-evaluation_file", default="evaluation.txt"); a("-no_consistency_eval", action="store_true")
+    a("-flow_pattern_eval", default=""); a("-occlusions_pattern_eval", default="")
+    a("-invert_occlusions_eval", action="store_true"); a("-backward_eval", action="store_true")
+    a("-content_weights", default="1.0"); a("-content_layers", default="16"); a("-loss_network", default=None)
+    a("-style_image", default=""); a("-style_image_size", type=int, default=256); a("-style_weights", default="5.0")
+    a("-style_layers", default="4,9,16,23"); a("-style_target_type", default="gram", choices=["gram", "mean"])
+    a("-fix_occlusions_eval", action="store_true")
+    # read by func_eval (:408-424) but never declared by the VR script; train_video.lua:33's option and default
+    a("-reliable_map_min_filter", type=int, default=7)
     a("-arch", default=core.synth.PAPER_ARCH)
     return p
 
@@ -69,6 +100,7 @@ def build_parser():
 class VRDriver:
     def __init__(self, opt):
         self.opt = opt
+        self.last_content = None
         self.last_segments = {}
         self.prev_last_segments = {}
         self.initialized = False
@@ -105,6 +137,12 @@ class VRDriver:
             r = opt.median_filter // 2
             self.equi_map = f32(vr_helper.make_cube_to_equirectangular_map(hplus - 2 * r, wplus - 2 * r, opt.overlap_pixel_w - r,
                                                                          opt.overlap_pixel_h - r, opt.out_equi_w, opt.out_equi_h))
+        if opt.evaluate:  # the min-filtered masks of evaluate_gradient (:408-424), indexed by mode
+            rr = opt.reliable_map_min_filter
+            mf = lambda m: (utils.min_filter(m, rr) if rr > 1 else m)[0].contiguous()
+            self.eval_mask = {1: mf(self.mask["left"]), 2: mf(self.mask["right"]), 3: mf(self.mask["right"] + self.mask["left"]),
+                              4: mf(self.mask_all)}
+            self.eval_mask[5] = self.eval_mask[4]
         self.initialized = True
 
     # ---- callbacks ---------------------------------------------------------------------------------------------
@@ -116,7 +154,8 @@ class VRDriver:
         img = load_image(path, 3)
         if not self.initialized:
             self._init(img.shape[1], img.shape[2])
-        return img.contiguous()
+        self.last_content = img.contiguous()  # :200, the content image of func_eval's perceptual term
+        return self.last_content
 
     def func_load_cert(self, opt, i, dtype):  # :204-237
         mode, file_idx = (i - 1) % 6, (i - 1) // 6 + opt.start_frame
@@ -185,6 +224,80 @@ class VRDriver:
     def func_is_single_image(self, i, opt):  # :304-310
         return i % 6 == 1 if opt.create_inconsistent else i == 1
 
+    # ---- -evaluate (:312-452) ----------------------------------------------------------------------------------------
+    def _trim(self, t):  # :321-325
+        oh, ow = self.opt.overlap_pixel_h // 2, self.opt.overlap_pixel_w // 2
+        return t[:, oh:self.hplus - oh, ow:self.wplus - ow]
+
+    @staticmethod
+    def _mse(a, b):  # nn.MSECriterion (mean), in double on the device
+        return float(((a.double() - b.double()) ** 2).mean())
+
+    def _edge(self, img1, img2):  # evaluate_edge(img1, img2, 'left') (:312-319)
+        return self._mse(img1[:, :, :1], img2[:, :, -1:])
+
+    def _edge_top(self, img2, edgeOther):  # evaluate_edge_top (:327-341): its first argument is never read
+        side1 = img2[:, :1, :]
+        if edgeOther == "left":
+            side2 = img2[:, :, :1].transpose(1, 2)
+        elif edgeOther == "right":
+            side2 = img2[:, :, -1:].transpose(1, 2).flip(2)
+        elif edgeOther == "top":
+            side2 = img2[:, :1, :].flip(1)  # reverses a size-1 dimension: side2 == side1
+        else:
+            side2 = img2[:, -1:, :]
+        return self._mse(side1, side2)
+
+    def _gradient(self, face, mask):  # evaluate_gradient (:344-387)
+        H, W = face.shape[-2:]
+        sums = torch.empty(6, dtype=torch.float64, device=face.device)
+        _lib.check(_lib.lib.fav_vr_eval_gradient(_lib.dptr(face.contiguous()), _lib.dptr(mask), H, W, _lib.dptr(sums),
+                                                 _lib.stream_ptr()))
+        return gradient_ratios(sums.tolist(), H, W)
+
+    def _load_flow_cert_eval(self, opt, file_idx, mode):  # load_flow_cert_eval (:389-401)
+        name = lambda pat: getFormatedFlowFileName(pat, file_idx - 1, file_idx, PROC_ORDER[mode])
+        flow = torch.from_numpy(flowFileLoader.load(name(opt.flow_pattern_eval or opt.flow_pattern))).cuda()
+        cert = load_image(name(opt.occlusions_pattern_eval or opt.occlusions_pattern), 1).cuda()
+        if opt.invert_occlusions_eval:
+            cert = 1.0 - cert
+        if opt.fix_occlusions_eval:  # fix_occlusions (:117-128): the displacement itself is tested against [0,H] x [0,W]
+            H, W = flow.shape[-2:]
+            out = (flow[0] < 0) | (flow[0] > H) | (flow[1] < 0) | (flow[1] > W)
+            cert = cert.masked_fill(out[None], 0.0)
+        return flow, cert
+
+    def func_eval(self, opt, i, func_percept_loss, dtype):  # :403-452
+        mode, file_idx = (i - 1) % 6, (i - 1) // 6 + 1  # file_idx without opt.start_frame, as written (:405)
+        ls = self.last_segments
+        gradx = grady = gradmag = edge = 0.0
+        if mode != 0:
+            gradx, grady, gradmag = self._gradient(ls[mode + 1], self.eval_mask[mode])
+        if mode == 1:
+            edge = self._edge(self._trim(ls[1]), self._trim(ls[2]))
+        elif mode == 2:
+            edge = self._edge(self._trim(ls[3]), self._trim(ls[1]))
+        elif mode == 3:  # the same pair twice (:415-416)
+            edge = (self._edge(self._trim(ls[2]), self._trim(ls[4])) + self._edge(self._trim(ls[2]), self._trim(ls[4]))) / 2
+        elif mode == 4:  # every term reads trim(last_segments[5]) only (:419-422)
+            t5 = self._trim(ls[5])
+            edge = (self._edge_top(t5, "top") + self._edge_top(t5, "right") + self._edge_top(t5, "left")
+                    + self._edge_top(t5, "bottom")) / 4
+        # (content, style) unpacked as `style_loss, content_loss` (:427), as in the plain driver; nan without a loss network
+        nan = float("nan")
+        style_loss, content_loss = func_percept_loss(self.last_content, ls[mode + 1]) if func_percept_loss else (nan, nan)
+        if i > 6 and not opt.no_consistency_eval:
+            flow, cert = self._load_flow_cert_eval(opt, file_idx, mode)
+            # at mode 5 func_save_image has already replaced prev_last_segments with this frame's re-blend (:530-532)
+            if opt.backward_eval:
+                t = utils.temporal_loss(ls[mode + 1], self.prev_last_segments[mode + 1], flow, cert)
+            else:
+                t = utils.temporal_loss(self.prev_last_segments[mode + 1], ls[mode + 1], flow, cert)
+            return [gradx, grady, gradmag, edge, style_loss, content_loss, t], 7
+        if opt.no_consistency_eval:
+            return [gradx, grady, gradmag, edge, style_loss, content_loss], 6
+        return [gradx, grady, gradmag, edge, style_loss, content_loss, 0.0], 7
+
     def blend_other_sides(self):  # :454-509 -- one fused kernel per face
         ls = self.last_segments
         plan = {1: [(2, "right", None), (3, "left", None), (5, "bottom", rotate180), (6, "top", rotate180)],
@@ -249,8 +362,12 @@ def main(argv=None, model_vid=None):
                             "writes (fast_artistic_video_vr.lua:524-526,576-584)")
     if opt.overlap_pixel_w % 2 or opt.overlap_pixel_h % 2:
         raise _lib.FavError(_lib.FAV_ERR_INVALID, "overlap_pixel_w/h must be even (the reference slices with overlap/2, :515-516)")
+    if opt.evaluate and opt.overlap_pixel_w != opt.overlap_pixel_h:
+        # evaluate_edge_top's MSECriterion compares a trimmed row with a trimmed column (:419-422): equal lengths only
+        raise _lib.FavError(_lib.FAV_ERR_INVALID, "-evaluate needs overlap_pixel_w == overlap_pixel_h (the mode-4 seam MSE compares "
+                            "a trimmed row with a trimmed column, fast_artistic_video_vr.lua:327-341,419-422)")
     d = VRDriver(opt)
-    core.run_fast_neural_video(opt, d.func_load_image, d.func_load_cert, None, d.func_make_last_frame_warped,
+    core.run_fast_neural_video(opt, d.func_load_image, d.func_load_cert, d.func_eval, d.func_make_last_frame_warped,
                                d.func_is_single_image, d.func_save_image, model_vid=model_vid)
     torch.cuda.synchronize()
     flush_saves()  # the PNGs of a VR frame are encoded on worker threads while the next frame's faces are stylized

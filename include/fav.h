@@ -150,6 +150,14 @@ FAV_API int fav_median_filter(const float *in, float *out, int C, int H, int W, 
 FAV_API int fav_vr_blend_sides(const float *base, const float *const sides[4], const float *const maps[4],
                                const int rot[4], const float *div, const float *mask, const float *anti_mask,
                                float *out, int S, void *stream);
+/* f-4  gradient metric of the VR driver's -evaluate   evaluate_gradient, fast_artistic_video_vr.lua:344-387
+ * face [3,H,W] fp32 (a stylized cube face, untrimmed), mask [H,W] fp32 (the min-filtered blend mask).  In double from the
+ * fp32 values: gx = max_c |f[c][y][x+2]-f[c][y][x]| on [H,W-2], gy = max_c |f[c][y+2][x]-f[c][y][x]| on [H-2,W];
+ * MX / MY = 3x3 stride-1 max-pool (padding cells ignored) of |m[y][x+2]-m[y][x]| / |m[y+2][x]-m[y][x]|.
+ * OVERWRITES the DEVICE doubles sums_dev[0..5] = { sum gx, sum gy, sum MX, sum MY, sum gx*MX, sum gy*MY }; the ratios
+ * gradx / grady / gradmag are formed from them by the caller.  Fixed summation order: bit-identical from call to call.
+ * H, W >= 3.  Per-CTA partials come from the stream's memory pool (cudaMallocAsync) and are freed on it. */
+FAV_API int fav_vr_eval_gradient(const float *face, const float *mask, int H, int W, double *sums_dev, void *stream);
 
 /* a-3 / a-13  Middlebury .flo (HOST side)          flowFileLoader.lua:17-37, consistencyChecker.cpp:16-36
  * layout 0: [dy,dx] (Lua loader order); layout 1: [u,v] (checker order). out: host [2,H,W] with room for capacity_floats
