@@ -335,6 +335,323 @@ __global__ void __launch_bounds__(256) percep_unpack_tap_kernel(const uint16_t *
   out[(int64_t)c * P + p] = __half2float(__ushort_as_half(hi[o])) + __half2float(__ushort_as_half(lo[o]));
 }
 
+// ---- backward (fav_percep_forward_backward) ---------------------------------------------------------------------------
+// The input gradient of a stride-1 convolution with pad (k-1)/2 is the same convolution geometry over the output gradient, with
+// the filters transposed and flipped: it runs on conv_tc_kernel like the forward.  Its operand is the fp16 hi/lo pair, whose
+// normal range starts at 6e-5 while the loss gradients sit near 1e-7 and shrink as they flow back, so every gradient operand is
+// packed multiplied by a per-tensor power of two that maps its max |g| into [2^14, 2^15).  The factor is exact, so it changes no
+// rounding; the kernel that reads the convolution's fp32 output divides it out.  The max lives in device memory.
+
+// 2^k for max |g| (float bits) in [2^(14-k), 2^(15-k)); 1 for an all-zero tensor.  |k| <= 126 keeps 2^k and 2^-k normal.
+__device__ __forceinline__ int grad_scale_exp(unsigned maxbits) {
+  if (maxbits == 0) return 0;
+  const int e = max((int)((maxbits >> 23) & 0xff), 1) - 127;  // floor(log2 max); subnormals as 2^-126
+  return min(max(14 - e, -126), 126);
+}
+__device__ __forceinline__ float grad_scale(unsigned maxbits) { return ldexpf(1.f, grad_scale_exp(maxbits)); }
+__device__ __forceinline__ float grad_unscale(unsigned maxbits) { return ldexpf(1.f, -grad_scale_exp(maxbits)); }
+
+// max of |v| over the block -> one atomicMax per warp on the float bits (an order-independent result)
+__device__ __forceinline__ void flush_absmax(float m, unsigned *out) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));
+}
+
+// net-space input [3][H][W] (BGR, 255 x - mean: what PerceptualCriterion:forward receives) -> the first convolution's operand
+__global__ void __launch_bounds__(128) percep_pack_net_kernel(const float *__restrict__ in, int H, int W, Operand dst) {
+  const int x = blockIdx.x * 128 + threadIdx.x, y = blockIdx.y;
+  if (x >= W) return;
+  const int64_t HW = (int64_t)H * W, p = (int64_t)y * W + x;
+  float v[8];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) v[c] = c < 3 ? __ldg(in + c * HW + p) : 0.f;
+  const int64_t o = dst.off16(dst.padT + y, 0, dst.padL + x);
+  split_store8(v, reinterpret_cast<uint4 *>(dst.hi) + o, reinterpret_cast<uint4 *>(dst.lo) + o);
+}
+
+// ContentLoss:updateGradInput (ContentLoss.lua:50-59, MSECriterion): g (+)= strength * 2 (F - F_t) / (C H W), one thread per (pixel, channel)
+__global__ void __launch_bounds__(256) percep_content_grad_kernel(const uint16_t *__restrict__ ah, const uint16_t *__restrict__ al,
+                                                                  const uint16_t *__restrict__ bh, const uint16_t *__restrict__ bl,
+                                                                  int Cp, int64_t P, float coef, int accumulate,
+                                                                  float *__restrict__ g) {
+  const int64_t p = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  const int c = blockIdx.y;
+  if (p >= P) return;
+  const int64_t o = ((p >> 3) * Cp + c) * 8 + (p & 7);
+  const float a = __half2float(__ushort_as_half(ah[o])) + __half2float(__ushort_as_half(al[o]));
+  const float b = __half2float(__ushort_as_half(bh[o])) + __half2float(__ushort_as_half(bl[o]));
+  const float v = coef * (a - b);
+  float *d = g + (int64_t)c * P + p;
+  *d = accumulate ? *d + v : v;
+}
+
+// StyleLoss 'mean' (two nn.Mean, StyleLoss.lua:57-67): g (+)= strength * 2 (mu_c - t_c) / C / (H W), broadcast over the pixels
+__global__ void __launch_bounds__(256) percep_mean_grad_kernel(const double *__restrict__ mu, const double *__restrict__ t, int64_t P,
+                                                               double coef, int accumulate, float *__restrict__ g) {
+  const int64_t p = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  const int c = blockIdx.y;
+  if (p >= P) return;
+  const float v = (float)(coef * (mu[c] - t[c]));
+  float *d = g + (int64_t)c * P + p;
+  *d = accumulate ? *d + v : v;
+}
+
+// D = strength * 4 (G - T) / (C^2 C H W), formed in double and rounded once (G and T are symmetric, so is D)
+__global__ void __launch_bounds__(256) percep_gram_diff_kernel(const double *__restrict__ G, const double *__restrict__ T, int n,
+                                                               double coef, float *__restrict__ D) {
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i < n) D[i] = (float)(coef * (G[i] - T[i]));
+}
+
+// GramMatrix:updateGradInput (GramMatrix.lua:54-78) after StyleLoss: g[c][p] (+)= sum_j D[c][j] F[j][p], F the tap (hi + lo).
+// CTA tile: 64 channels x 128 pixels, K = 16 channels per shared-memory step; thread: 4 channels x 8 pixels (p = tp + 16 i), fp32.
+// Every output element is written by one thread, with a fixed summation order.
+constexpr int kGbM = 64, kGbN = 128, kGbK = 16;
+__global__ void __launch_bounds__(256) percep_gram_grad_kernel(const float *__restrict__ D, const uint4 *__restrict__ hi,
+                                                               const uint4 *__restrict__ lo, int C, int Cp, int64_t P, int accumulate,
+                                                               float *__restrict__ g) {
+  __shared__ float As[kGbK][kGbM];
+  __shared__ float Bs[kGbK][kGbN];
+  const int t = threadIdx.x, tc = t >> 4, tp = t & 15;
+  const int c0 = blockIdx.y * kGbM;
+  const int64_t p0 = (int64_t)blockIdx.x * kGbN;
+  float acc[4][8];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+  for (int j0 = 0; j0 < C; j0 += kGbK) {
+    {  // A: D[j0 + k][c0 + 4 q + i] (= D[c][j], symmetric)
+      const int k = t >> 4, q = t & 15, j = j0 + k;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = c0 + 4 * q + i;
+        As[k][4 * q + i] = (j < C && c < C) ? __ldg(D + (int64_t)j * C + c) : 0.f;
+      }
+    }
+    {  // B: F[j0 + k][p0 + 8 b .. + 8]: one 16-byte hi / lo unit of the tap layout [P/8][Cp][8]
+      const int k = t >> 4, b = t & 15, j = j0 + k;
+      float v[8];
+      const int64_t kb = (p0 >> 3) + b;
+      if (j < Cp && (kb << 3) < P) {
+        join8(__ldg(hi + kb * Cp + j), __ldg(lo + kb * Cp + j), v);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = 0.f;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) Bs[k][8 * b + i] = v[i];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < kGbK; ++k) {
+      float a[4], b[8];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = As[k][4 * tc + i];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) b[j] = Bs[k][tp + 16 * j];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int c = c0 + 4 * tc + i;
+    if (c >= C) continue;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int64_t p = p0 + tp + 16 * j;
+      if (p >= P) continue;
+      float *d = g + (int64_t)c * P + p;
+      *d = accumulate ? *d + acc[i][j] : acc[i][j];
+    }
+  }
+}
+
+// One stage of the backward pass: the gradient at the raw output of conv s (bias included), from
+//  - the gradient at the input of conv s + 1 (the fp32 output of its input-gradient convolution, scaled by 2^k), and
+//  - the gradient of every loss layer of this stage (planar fp32 [C][H][W] at the loss layer's own size),
+// each passed back through the modules between conv s and its place: max-pooling as a gather (each pixel sums the windows whose
+// first maximum in row-major order it is; no atomics), ReLU as the mask raw > 0 (nn.ReLU(true): its input is its output, and
+// max-pooling commutes with the ReLU, so pooled-then-rectified terms use the same mask).  One thread per (pixel, channel quad).
+constexpr int kMaxStageTerms = 8;
+struct BwdTerm {
+  const float *g;  // planar [C][H][W]; null for the next-stage term, which reads `nxt`
+  int H, W, relu, pool;
+};
+struct BwdStage {
+  const float4 *raw;
+  int C, Cq, Wp, H, W;
+  PoolSpec pool;          // the stage's max-pooling (pooled terms)
+  const float4 *nxt;      // next-stage term: raw layout, nxt_Wp pitch, the same channel quads; null at the deepest stage
+  int nxt_Wp;
+  const unsigned *nxt_max;
+  int nt;
+  BwdTerm t[kMaxStageTerms];
+  float4 *out;            // raw layout (Cq, Wp)
+  unsigned *out_max;
+};
+
+__device__ __forceinline__ void term_at(const BwdStage &s, const BwdTerm &tm, int cq, int y, int x, float inv, float v[4]) {
+  if (!tm.g) {
+    const float4 a = __ldg(s.nxt + ((int64_t)y * s.Cq + cq) * s.nxt_Wp + x);
+    v[0] = a.x * inv; v[1] = a.y * inv; v[2] = a.z * inv; v[3] = a.w * inv;
+    return;
+  }
+  const int64_t HW = (int64_t)tm.H * tm.W, p = (int64_t)y * tm.W + x;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) v[i] = 4 * cq + i < s.C ? __ldg(tm.g + (4 * cq + i) * HW + p) : 0.f;
+}
+
+__global__ void __launch_bounds__(128) percep_bwd_stage_kernel(const BwdStage s) {
+  const int x = blockIdx.x * 128 + threadIdx.x, y = blockIdx.y, cq = blockIdx.z;
+  float m = 0.f;
+  if (x < s.W) {
+    const float inv = s.nxt ? grad_unscale(*s.nxt_max) : 0.f;
+    float ap[4] = {0.f, 0.f, 0.f, 0.f}, ar[4] = {0.f, 0.f, 0.f, 0.f};  // unmasked / ReLU-masked sums
+    bool pooled = false;
+    for (int k = 0; k < s.nt; ++k) {
+      const BwdTerm &tm = s.t[k];
+      if (tm.pool) { pooled = true; continue; }
+      float v[4];
+      term_at(s, tm, cq, y, x, inv, v);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) (tm.relu ? ar : ap)[i] += v[i];
+    }
+    if (pooled) {
+      const PoolSpec &pl = s.pool;
+      const int oy0 = max(0, (y + pl.ph - pl.kh + pl.sh) / pl.sh), oy1 = (y + pl.ph) / pl.sh;
+      const int ox0 = max(0, (x + pl.pw - pl.kw + pl.sw) / pl.sw), ox1 = (x + pl.pw) / pl.sw;
+      // the pooled grid: every pooled term has the same extents (BwdTerm H / W)
+      int Ho = 0, Wo = 0;
+      for (int k = 0; k < s.nt; ++k)
+        if (s.t[k].pool) { Ho = s.t[k].H; Wo = s.t[k].W; break; }
+      for (int oy = oy0; oy <= min(oy1, Ho - 1); ++oy)
+        for (int ox = ox0; ox <= min(ox1, Wo - 1); ++ox) {
+          const int hs = oy * pl.sh - pl.ph, ws = ox * pl.sw - pl.pw;
+          const int he = min(hs + pl.kh, s.H), we = min(ws + pl.kw, s.W);
+          float best[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+          int bi[4] = {-1, -1, -1, -1};
+          for (int iy = max(hs, 0); iy < he; ++iy)
+            for (int ix = max(ws, 0); ix < we; ++ix) {
+              const float4 a = __ldg(s.raw + ((int64_t)iy * s.Cq + cq) * s.Wp + ix);
+              const float av[4] = {a.x, a.y, a.z, a.w};
+              const int id = iy * s.W + ix;
+#pragma unroll
+              for (int i = 0; i < 4; ++i)
+                if (av[i] > best[i]) { best[i] = av[i]; bi[i] = id; }
+            }
+          const int self = y * s.W + x;
+          if (bi[0] != self && bi[1] != self && bi[2] != self && bi[3] != self) continue;
+          for (int k = 0; k < s.nt; ++k) {
+            const BwdTerm &tm = s.t[k];
+            if (!tm.pool) continue;
+            float v[4];
+            term_at(s, tm, cq, oy, ox, inv, v);
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+              if (bi[i] == self) (tm.relu ? ar : ap)[i] += v[i];
+          }
+        }
+    }
+    const float4 r = __ldg(s.raw + ((int64_t)y * s.Cq + cq) * s.Wp + x);
+    const float rv[4] = {r.x, r.y, r.z, r.w};
+    float g[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      g[i] = 4 * cq + i < s.C ? ap[i] + (rv[i] > 0.f ? ar[i] : 0.f) : 0.f;
+      m = fmaxf(m, fabsf(g[i]));
+    }
+    s.out[((int64_t)y * s.Cq + cq) * s.Wp + x] = make_float4(g[0], g[1], g[2], g[3]);
+  }
+  flush_absmax(m, s.out_max);
+}
+
+// gradient (raw layout) x 2^k -> the input-gradient convolution's operand (fp16 hi / lo, zero border kept)
+__global__ void __launch_bounds__(128) percep_bwd_pack_kernel(const float4 *__restrict__ g, int Cq, int Wp, const unsigned *gmax,
+                                                              Operand dst) {
+  const int x = blockIdx.x * 128 + threadIdx.x, y = blockIdx.y, cb = blockIdx.z;
+  if (x >= dst.W) return;
+  const float sc = grad_scale(*gmax);
+  const float4 a = __ldg(g + ((int64_t)y * Cq + 2 * cb) * Wp + x);
+  const float4 b = 2 * cb + 1 < Cq ? __ldg(g + ((int64_t)y * Cq + 2 * cb + 1) * Wp + x) : make_float4(0.f, 0.f, 0.f, 0.f);
+  float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = cb * 8 + i < dst.C ? v[i] * sc : 0.f;
+  const int64_t o = dst.off16(dst.padT + y, cb, dst.padL + x);
+  split_store8(v, reinterpret_cast<uint4 *>(dst.hi) + o, reinterpret_cast<uint4 *>(dst.lo) + o);
+}
+
+// the first convolution's input gradient (raw layout, 2^k scaled) -> grad_input [3][H][W] fp32
+__global__ void __launch_bounds__(256) percep_grad_input_kernel(const float4 *__restrict__ d, int Wp, const unsigned *gmax, int H, int W,
+                                                                float *__restrict__ out) {
+  const int64_t p = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (p >= (int64_t)H * W) return;
+  const int y = (int)(p / W), x = (int)(p - (int64_t)y * W);
+  const float inv = grad_unscale(*gmax);
+  const float4 a = __ldg(d + (int64_t)y * Wp + x);  // Cq = 1
+  const int64_t HW = (int64_t)H * W;
+  out[p] = a.x * inv;
+  out[HW + p] = a.y * inv;
+  out[2 * HW + p] = a.z * inv;
+}
+
+// ---- pixel loss and TotalVariation gradients (train_video.lua:117-126,354-366; TotalVariation.lua:19-35) -------------
+// pixel_crit:forward / backward(out2 .* cert, prev_warped_masked): per-element loss terms and d loss / d (out2 .* cert), added to
+// grad_accum WITHOUT the certainty factor (train_video.lua:357-364 adds the criterion's gradInput as it is).  type 0 L2 (MSE),
+// 1 L1 (AbsCriterion), 2 SmoothL1; sizeAverage over N*3*H*W (norm: the criterion's fp32 2/n or 1/n), then x weight as
+// grad_out:add(weight, grad_pix).  Per-block loss partials in double, summed in a fixed order.
+__global__ void __launch_bounds__(kRedThreads) fav_pixel_loss_grad_kernel(const float *__restrict__ out2, const float *__restrict__ prev,
+                                                                          const float *__restrict__ cert, int64_t HW, int64_t n, int type,
+                                                                          float norm, float weight, float *__restrict__ acc,
+                                                                          double *__restrict__ partial) {
+  __shared__ double sh[kRedThreads];
+  double s = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * kRedThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kRedThreads) {
+    const int64_t img = i / (3 * HW), pix = (i - img * 3 * HW) % HW;
+    const float a = __fmul_rn(out2[i], __ldg(cert + img * HW + pix));
+    const float d = __fsub_rn(a, prev[i]);
+    double l;
+    float g;
+    if (type == 0) { l = (double)d * d; g = __fmul_rn(norm, d); }
+    else if (type == 1) { l = fabs((double)d); g = d >= 0.f ? norm : -norm; }
+    else {
+      const double z = fabs((double)d);
+      l = z < 1.0 ? 0.5 * z * z : z - 0.5;
+      g = d < -1.f ? -norm : (d > 1.f ? norm : __fmul_rn(norm, d));
+    }
+    s += l;
+    acc[i] = __fadd_rn(acc[i], __fmul_rn(weight, g));
+  }
+  const double r = block_sum<kRedThreads>(s, sh);
+  if (threadIdx.x == 0) partial[blockIdx.x] = r;
+}
+
+// TotalVariation:updateGradInput with its {1,-2} ranges, as a gather, in the module's fp32 order: diffs on the (H-1) x (W-1)
+// corner, added into zero, then strength x, then added to grad_accum (the module's gradOutput)
+__global__ void __launch_bounds__(256) fav_tv_grad_kernel(const float *__restrict__ x, int64_t planes, int H, int W, float strength,
+                                                          float *__restrict__ acc) {
+  const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  const int64_t HW = (int64_t)H * W;
+  if (i >= planes * HW) return;
+  const int64_t pl = i / HW;
+  const int p = (int)(i - pl * HW), yy = p / W, xx = p - yy * W;
+  const float *X = x + pl * HW;
+  auto at = [&](int y, int xc) { return X[(int64_t)y * W + xc]; };
+  float t = 0.f;
+  if (yy < H - 1 && xx < W - 1) {
+    t = t + (at(yy, xx) - at(yy, xx + 1));
+    t = t + (at(yy, xx) - at(yy + 1, xx));
+  }
+  if (yy < H - 1 && xx >= 1) t = t - (at(yy, xx - 1) - at(yy, xx));
+  if (yy >= 1 && xx < W - 1) t = t - (at(yy - 1, xx) - at(yy, xx));
+  acc[i] = __fadd_rn(acc[i], __fmul_rn(t, strength));
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 struct PModule {
@@ -351,6 +668,10 @@ struct PConv {
   bool set = false;
   std::vector<ConvDef> blocks;        // one per 128-channel N block
   std::vector<float *> d_bias;        // per block, Npad entries
+  // input gradient (fav_percep_forward_backward): a cout -> cin convolution with the flipped, transposed filters and zero
+  // bias, one ConvDef per 128-channel N block of cin; packed on the first backward call
+  std::vector<ConvDef> dblocks;
+  float *d_zero = nullptr;            // kMaxNBlock zero biases
 };
 
 struct PTapSpec {  // a loss layer's feature map: (relu, pool) applied to the raw output of conv `stage`
@@ -382,6 +703,14 @@ struct PPlan {
   size_t gram_part_floats = 0;
   double *red = nullptr;               // reduction partials
   int *overflow = nullptr;
+  // backward plans only (build_pplan retain): every raw above has its own buffer, and the gradient buffers
+  std::vector<Operand> gop;            // [conv s]: operand of its input-gradient convolution (output gradient x 2^k)
+  std::vector<RawTensor> gin;          // [conv s]: that convolution's fp32 output, the gradient at conv s's input (one buffer)
+  std::vector<std::vector<ConvJob>> djobs;
+  float *gbuf = nullptr;               // one stage's output gradient, raw layout
+  std::vector<float *> tgrad;          // [tap]: gradient of the loss layers there, planar [C][H][W]
+  float *gram_d = nullptr;             // C x C: strength * 4 (G - T) / (C^2 C H W) of one style layer
+  unsigned *gmax = nullptr;            // [conv s]: max |gradient| at its output (float bits)
   std::vector<void *> allocs;
   ~PPlan() {
     for (void *p : allocs) cudaFree(p);
@@ -411,13 +740,17 @@ struct fav_percep {
   bool finalized = false;
   bool has_target = false;
   int num_sms = 132;
+  int bwd_refuse = 0;             // first convolution module whose input gradient is not the same-geometry convolution
+  bool bwd_ready = false;         // dblocks packed
   std::map<std::pair<int, int>, std::unique_ptr<PPlan>> plans;
+  std::map<std::pair<int, int>, std::unique_ptr<PPlan>> bplans;  // fav_percep_forward_backward: raw outputs kept
   PPlan *last_plan = nullptr;
   std::vector<double *> target, stat;  // per style layer: aggregate of the style image / of the last evaluated image
   double *d_losses = nullptr;          // [n_content + n_style]
   std::vector<void *> allocs;
   ~fav_percep() {
     plans.clear();
+    bplans.clear();
     for (void *p : allocs) cudaFree(p);
   }
 };
@@ -444,10 +777,14 @@ static int tap_size(const PTapSpec &t, const std::vector<RawTensor> &raw, int *H
   return FAV_OK;
 }
 
-static int build_pplan(fav_percep *P, int H, int W, PPlan **out) {
+static int build_backward(fav_percep *P, PPlan &pl);
+
+// retain: a backward plan (P->bplans) -- every convolution's raw output in its own buffer, plus the gradient buffers
+static int build_pplan(fav_percep *P, int H, int W, PPlan **out, bool retain = false) {
+  auto &plans = retain ? P->bplans : P->plans;
   auto key = std::make_pair(H, W);
-  auto it = P->plans.find(key);
-  if (it != P->plans.end()) { *out = it->second.get(); return FAV_OK; }
+  auto it = plans.find(key);
+  if (it != plans.end()) { *out = it->second.get(); return FAV_OK; }
   FAV_REQUIRE(H >= 1 && W >= 1, "fav_percep: bad image size %dx%d", W, H);
   std::unique_ptr<PPlan> pl(new PPlan());
   pl->H = H; pl->W = W;
@@ -479,9 +816,13 @@ static int build_pplan(fav_percep *P, int H, int W, PPlan **out) {
       }
     }
   }
-  float *raw_buf = nullptr;
-  FAV_TRY(p_alloc(pl->allocs, (void **)&raw_buf, raw_max * sizeof(float) + 4096));
-  for (RawTensor &r : pl->raw) r.p = raw_buf;
+  if (retain) {
+    for (RawTensor &r : pl->raw) FAV_TRY(p_alloc(pl->allocs, (void **)&r.p, (size_t)r.Hp * r.Cq * r.Wp * 4 * sizeof(float) + 4096));
+  } else {
+    float *raw_buf = nullptr;
+    FAV_TRY(p_alloc(pl->allocs, (void **)&raw_buf, raw_max * sizeof(float) + 4096));
+    for (RawTensor &r : pl->raw) r.p = raw_buf;
+  }
   for (int s = 0; s < ns; ++s) {
     Operand &o = pl->in[s];
     FAV_TRY(p_alloc(pl->allocs, (void **)&o.hi, o.elems16 * 16));
@@ -534,8 +875,66 @@ static int build_pplan(fav_percep *P, int H, int W, PPlan **out) {
   pl->gram_part_floats = part_max;
   FAV_TRY(p_alloc(pl->allocs, (void **)&pl->red, (size_t)kRedBlocks * sizeof(double)));
   FAV_TRY(p_alloc(pl->allocs, (void **)&pl->overflow, sizeof(int)));
+  if (retain) FAV_TRY(build_backward(P, *pl));
   *out = pl.get();
-  P->plans[key] = std::move(pl);
+  plans[key] = std::move(pl);
+  return FAV_OK;
+}
+
+// the gradient side of a backward plan: per conv s the operand of its input-gradient convolution (at conv s's output size, the
+// padding of the dgrad ConvDef) and that convolution's jobs writing into one shared fp32 buffer; per tap a planar loss gradient
+static int build_backward(fav_percep *P, PPlan &pl) {
+  const int ns = (int)P->convs.size();
+  size_t graw = 16, draw = 16;
+  pl.gop.resize(ns); pl.gin.resize(ns); pl.djobs.resize(ns);
+  for (int s = 0; s < ns; ++s) {
+    const PConv &pc = P->convs[s];
+    const RawTensor &r = pl.raw[s];
+    Operand &o = pl.gop[s];
+    o = operand_geometry(pc.cout, r.H, r.W, &pc.dblocks[0]);
+    FAV_TRY(p_alloc(pl.allocs, (void **)&o.hi, o.elems16 * 16));
+    FAV_TRY(p_alloc(pl.allocs, (void **)&o.lo, o.elems16 * 16));
+    RawTensor &d = pl.gin[s];
+    d.C = pc.cin; d.Cq = round_up(pc.cin, 4) / 4; d.H = pl.in[s].H; d.W = pl.in[s].W; d.Hp = d.H + 2; d.Wp = round_up(d.W, kTileM);
+    graw = std::max(graw, (size_t)r.Hp * r.Cq * r.Wp * 4);
+    draw = std::max(draw, (size_t)d.Hp * d.Cq * d.Wp * 4);
+  }
+  float *dbuf = nullptr;
+  FAV_TRY(p_alloc(pl.allocs, (void **)&pl.gbuf, graw * sizeof(float) + 4096));
+  FAV_TRY(p_alloc(pl.allocs, (void **)&dbuf, draw * sizeof(float) + 4096));
+  for (int s = 0; s < ns; ++s) {
+    PConv &pc = P->convs[s];
+    RawTensor &d = pl.gin[s];
+    d.p = dbuf;
+    for (size_t b = 0; b < pc.dblocks.size(); ++b) {
+      ConvDef &c = pc.dblocks[b];
+      ConvJob j;
+      int ho, wo;
+      conv_out_size(c, pl.gop[s].H, pl.gop[s].W, &ho, &wo);
+      if (ho != d.H || wo != d.W || fill_conv_job(c, c.phases[0], pl.gop[s], j) != FAV_OK) {
+        set_error("loss network: module %d (convolution): its input gradient has no tensor-core plan", pc.module);
+        return FAV_ERR_UNSUPPORTED;
+      }
+      j.b = c.phases[0].d_b_tc; j.bias = pc.d_zero;
+      j.raw = d.p + conv_nblock_raw_offset((int)b, d.Wp); j.raw_Cq = d.Cq; j.raw_Wp = d.Wp;
+      j.final_mode = 0;
+      conv_tc_choose_slots(j);
+      if (conv_tc_smem_bytes(j) > 227 * 1024 || (!j.b_resident && j.b_slots < 2)) {
+        set_error("loss network: module %d (convolution): input gradient exceeds the shared memory budget", pc.module);
+        return FAV_ERR_UNSUPPORTED;
+      }
+      pl.djobs[s].push_back(j);
+    }
+  }
+  size_t dmax = 16;
+  for (const PTap &tp : pl.taps[1]) {
+    float *g = nullptr;
+    FAV_TRY(p_alloc(pl.allocs, (void **)&g, (size_t)tp.C * tp.H * tp.W * sizeof(float)));
+    pl.tgrad.push_back(g);
+    dmax = std::max(dmax, (size_t)tp.C * tp.C);
+  }
+  FAV_TRY(p_alloc(pl.allocs, (void **)&pl.gram_d, dmax * sizeof(float)));
+  FAV_TRY(p_alloc(pl.allocs, (void **)&pl.gmax, (size_t)ns * sizeof(unsigned)));
   return FAV_OK;
 }
 
@@ -546,14 +945,20 @@ static int launch_pack_tap(const RawTensor &r, const PTapSpec &t, const PTap &tp
   return post_launch("percep_pack_tap");
 }
 
-// one forward of the loss network: pass 0 stops after the deepest content layer and keeps the content taps only
-static int run_pass(fav_percep *P, PPlan &pl, const float *rgb, int pass, cudaStream_t st) {
+// one forward of the loss network: pass 0 stops after the deepest content layer and keeps the content taps only.
+// img: RGB in [0,1] (the VGG preprocess fused into the first pack), or, net_space, the preprocessed BGR image itself
+static int run_pass(fav_percep *P, PPlan &pl, const float *img, int pass, cudaStream_t st, bool net_space = false) {
   const int ns = (int)P->convs.size();
   const int last = pass == 0 ? P->last_content_stage : ns - 1;
   {
     const Operand &o = pl.in[0];
-    percep_pack_rgb_kernel<<<dim3(ceil_div(pl.W, 128), pl.H), 128, 0, st>>>(rgb, pl.H, pl.W, o);
-    FAV_TRY(post_launch("percep_pack_rgb"));
+    if (net_space) {
+      percep_pack_net_kernel<<<dim3(ceil_div(pl.W, 128), pl.H), 128, 0, st>>>(img, pl.H, pl.W, o);
+      FAV_TRY(post_launch("percep_pack_net"));
+    } else {
+      percep_pack_rgb_kernel<<<dim3(ceil_div(pl.W, 128), pl.H), 128, 0, st>>>(img, pl.H, pl.W, o);
+      FAV_TRY(post_launch("percep_pack_rgb"));
+    }
   }
   for (int s = 0; s <= last; ++s) {
     for (const ConvJob &j : pl.jobs[s]) FAV_TRY(launch_conv_tc(j, P->num_sms, st));
@@ -604,6 +1009,163 @@ static int check_overflow(PPlan &pl, cudaStream_t st) {
     return FAV_ERR_UNSUPPORTED;
   }
   return FAV_OK;
+}
+
+// MSE of every loss layer after the two passes -> P->d_losses (content layers, then style layers)
+static int launch_losses(fav_percep *p, PPlan &pl, cudaStream_t st) {
+  const size_t nc = p->content_tap.size(), nsty = p->style_tap.size();
+  for (size_t k = 0; k < nc; ++k) {  // nn.MSECriterion: mean over C*H*W
+    const PTap &a = pl.taps[1][p->content_tap[k]], &b = pl.taps[0][p->content_tap[k]];
+    percep_sqdiff_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(a.hi, a.lo, b.hi, b.lo, a.nkb * a.Cp, pl.red);
+    FAV_TRY(post_launch("percep_sqdiff"));
+    percep_sum_kernel<<<1, kRedThreads, 0, st>>>(pl.red, kRedBlocks, 1.0 / ((double)a.C * a.H * a.W), p->d_losses + k);
+    FAV_TRY(post_launch("percep_sum"));
+  }
+  for (size_t k = 0; k < nsty; ++k) {  // nn.MSECriterion over the C x C Gram matrix (or the C means)
+    const PTap &a = pl.taps[1][p->style_tap[k]];
+    FAV_TRY(aggregate(p, pl, a, p->stat[k], st));
+    const int n = agg_len(p, a.C);
+    percep_vec_sqdiff_kernel<<<1, kRedThreads, 0, st>>>(p->stat[k], p->target[k], n, 1.0 / n, p->d_losses + nc + k);
+    FAV_TRY(post_launch("percep_vec_sqdiff"));
+  }
+  return FAV_OK;
+}
+
+// P->d_losses -> host (synchronises), the overflow check, strength * MSE per layer and the two totals in layer order
+// (PerceptualCriterion.lua:141-152)
+static int finish_losses(fav_percep *p, PPlan &pl, cudaStream_t st, double *content_loss, double *style_loss, double *layer_losses) {
+  const size_t nc = p->content_tap.size(), nsty = p->style_tap.size();
+  std::vector<double> mse(nc + nsty + 1, 0.0);
+  FAV_TRY(check_cuda(cudaMemcpyAsync(mse.data(), p->d_losses, mse.size() * sizeof(double), cudaMemcpyDeviceToHost, st),
+                     "cudaMemcpyAsync(losses)"));
+  FAV_TRY(check_overflow(pl, st));
+  double tc = 0.0, ts = 0.0;
+  for (size_t k = 0; k < nc; ++k) tc += p->content_w[k] * mse[k];
+  for (size_t k = 0; k < nsty; ++k) ts += p->style_w[k] * mse[nc + k];
+  if (layer_losses) {
+    for (size_t k = 0; k < nc; ++k) layer_losses[k] = p->content_w[k] * mse[k];
+    for (size_t k = 0; k < nsty; ++k) layer_losses[nc + k] = p->style_w[k] * mse[nc + k];
+  }
+  *content_loss = tc;
+  *style_loss = ts;
+  return FAV_OK;
+}
+
+// host-only: the first convolution whose input gradient is not a same-geometry convolution (stride 1, pad (k-1)/2), 0 if none
+static int bwd_unsupported_module(const fav_percep *P) {
+  for (const PConv &pc : P->convs)
+    if (pc.stride != 1 || pc.pad != (pc.k - 1) / 2) return pc.module;
+  return 0;
+}
+
+// the input-gradient convolutions: W'[ci][co][ky][kx] = W[co][ci][k-1-ky][k-1-kx], a [cin][cout][k][k] tensor read as the
+// weights of a cout -> cin convolution, packed per 128-channel N block of cin like the forward's
+static int prepare_backward(fav_percep *P) {
+  if (P->bwd_ready) return FAV_OK;
+  for (PConv &pc : P->convs) {
+    const int k = pc.k;
+    std::vector<float> wt((size_t)pc.cin * pc.cout * k * k);
+    for (int co = 0; co < pc.cout; ++co)
+      for (int ci = 0; ci < pc.cin; ++ci)
+        for (int ky = 0; ky < k; ++ky)
+          for (int kx = 0; kx < k; ++kx)
+            wt[(((size_t)ci * pc.cout + co) * k + ky) * k + kx] = pc.w[(((size_t)co * pc.cin + ci) * k + (k - 1 - ky)) * k + (k - 1 - kx)];
+    std::vector<ConvDef> blocks;
+    for (int b = 0; b < conv_nblocks(pc.cin); ++b) {
+      ConvDef c;
+      init_nblock_conv_def(c, "percep_dgrad" + std::to_string(pc.module), pc.cout, pc.cin, k, 1, pc.pad, b);
+      if (build_phase_tables(c, c.phases[0]) != FAV_OK) {
+        set_error("loss network module %d: the input gradient (convolution %d->%d k%d) is not a geometry the tensor-core planner runs",
+                  pc.module, pc.cout, pc.cin, k);
+        return FAV_ERR_UNSUPPORTED;
+      }
+      std::vector<uint16_t> pk = pack_phase_weights(c, c.phases[0], conv_nblock_weights(wt, pc.cout, pc.cin, k, b));
+      void *d = nullptr;
+      FAV_TRY(p_alloc(P->allocs, &d, pk.size() * 2));
+      FAV_TRY(check_cuda(cudaMemcpy(d, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice), "cudaMemcpy(percep dgrad weights)"));
+      c.phases[0].d_b_tc = reinterpret_cast<uint4 *>(d);
+      blocks.push_back(std::move(c));
+    }
+    if (!pc.d_zero) FAV_TRY(p_alloc(P->allocs, (void **)&pc.d_zero, kMaxNBlock * sizeof(float)));
+    pc.dblocks = std::move(blocks);
+  }
+  P->bwd_ready = true;
+  return FAV_OK;
+}
+
+// PerceptualCriterion:updateGradInput (PerceptualCriterion.lua:158-161): the loss layers' gradients, then from the deepest
+// convolution back to the input.  Stage s: gradient at conv s's raw output (percep_bwd_stage_kernel), x 2^k into the operand of its
+// input-gradient convolution, which writes the (scaled) gradient at conv s's input for stage s - 1 or grad_input.
+static int run_backward(fav_percep *P, PPlan &pl, float *grad_input, cudaStream_t st) {
+  const int ns = (int)P->convs.size();
+  std::vector<int> written(P->taps.size(), 0);
+  for (size_t k = 0; k < P->content_tap.size(); ++k) {
+    const int t = P->content_tap[k];
+    const PTap &a = pl.taps[1][t], &b = pl.taps[0][t];
+    const int64_t HW = (int64_t)a.H * a.W;
+    const float coef = (float)(P->content_w[k] * 2.0 / ((double)a.C * HW));
+    percep_content_grad_kernel<<<dim3((unsigned)ceil_div64(HW, 256), a.C), 256, 0, st>>>(
+        reinterpret_cast<const uint16_t *>(a.hi), reinterpret_cast<const uint16_t *>(a.lo), reinterpret_cast<const uint16_t *>(b.hi),
+        reinterpret_cast<const uint16_t *>(b.lo), a.Cp, HW, coef, written[t], pl.tgrad[t]);
+    FAV_TRY(post_launch("percep_content_grad"));
+    written[t] = 1;
+  }
+  for (size_t k = 0; k < P->style_tap.size(); ++k) {
+    const int t = P->style_tap[k];
+    const PTap &a = pl.taps[1][t];
+    const int64_t HW = (int64_t)a.H * a.W;
+    if (P->agg == 1) {
+      percep_mean_grad_kernel<<<dim3((unsigned)ceil_div64(HW, 256), a.C), 256, 0, st>>>(
+          P->stat[k], P->target[k], HW, P->style_w[k] * 2.0 / ((double)a.C * HW), written[t], pl.tgrad[t]);
+      FAV_TRY(post_launch("percep_mean_grad"));
+    } else {
+      const double C = a.C;
+      percep_gram_diff_kernel<<<ceil_div(a.C * a.C, 256), 256, 0, st>>>(P->stat[k], P->target[k], a.C * a.C,
+                                                                        P->style_w[k] * 4.0 / (C * C * C * (double)HW), pl.gram_d);
+      FAV_TRY(post_launch("percep_gram_diff"));
+      percep_gram_grad_kernel<<<dim3((unsigned)ceil_div64(HW, kGbN), ceil_div(a.C, kGbM)), 256, 0, st>>>(
+          pl.gram_d, a.hi, a.lo, a.C, a.Cp, HW, written[t], pl.tgrad[t]);
+      FAV_TRY(post_launch("percep_gram_grad"));
+    }
+    written[t] = 1;
+  }
+  FAV_TRY(check_cuda(cudaMemsetAsync(pl.gmax, 0, (size_t)ns * sizeof(unsigned), st), "cudaMemsetAsync(gmax)"));
+  for (int s = ns - 1; s >= 0; --s) {
+    const RawTensor &r = pl.raw[s];
+    BwdStage bs;
+    memset(&bs, 0, sizeof(bs));
+    bs.raw = reinterpret_cast<const float4 *>(r.p); bs.C = r.C; bs.Cq = r.Cq; bs.Wp = r.Wp; bs.H = r.H; bs.W = r.W;
+    if (s + 1 < ns) {
+      const PStageSpec &nx = P->next[s];
+      const RawTensor &d = pl.gin[s + 1];
+      bs.nxt = reinterpret_cast<const float4 *>(d.p); bs.nxt_Wp = d.Wp; bs.nxt_max = pl.gmax + s + 1;
+      bs.t[bs.nt++] = BwdTerm{nullptr, d.H, d.W, nx.relu, nx.pool.on};
+      if (nx.pool.on) bs.pool = nx.pool;
+    }
+    for (size_t t = 0; t < P->taps.size(); ++t) {
+      const PTapSpec &ts = P->taps[t];
+      if (ts.stage != s) continue;
+      if (bs.nt == kMaxStageTerms) {
+        set_error("loss network: more than %d loss layers between two convolutions", kMaxStageTerms - 1);
+        return FAV_ERR_UNSUPPORTED;
+      }
+      const PTap &tp = pl.taps[1][t];
+      bs.t[bs.nt++] = BwdTerm{pl.tgrad[t], tp.H, tp.W, ts.relu, ts.pool.on};
+      if (ts.pool.on) bs.pool = ts.pool;
+    }
+    bs.out = reinterpret_cast<float4 *>(pl.gbuf); bs.out_max = pl.gmax + s;
+    percep_bwd_stage_kernel<<<dim3(ceil_div(r.W, 128), r.H, r.Cq), 128, 0, st>>>(bs);
+    FAV_TRY(post_launch("percep_bwd_stage"));
+    const Operand &o = pl.gop[s];
+    percep_bwd_pack_kernel<<<dim3(ceil_div(o.W, 128), o.H, o.Cb), 128, 0, st>>>(reinterpret_cast<const float4 *>(pl.gbuf), r.Cq, r.Wp,
+                                                                                pl.gmax + s, o);
+    FAV_TRY(post_launch("percep_bwd_pack"));
+    for (const ConvJob &j : pl.djobs[s]) FAV_TRY(launch_conv_tc(j, P->num_sms, st));
+  }
+  const RawTensor &d = pl.gin[0];
+  percep_grad_input_kernel<<<(unsigned)ceil_div64((int64_t)pl.H * pl.W, 256), 256, 0, st>>>(
+      reinterpret_cast<const float4 *>(d.p), d.Wp, pl.gmax, pl.H, pl.W, grad_input);
+  return post_launch("percep_grad_input");
 }
 
 }  // namespace fav
@@ -820,32 +1382,71 @@ int fav_percep_evaluate(fav_percep_t *p, const float *content, const float *styl
   // PerceptualCriterion.lua:85-93 then :117-155: capture the content targets, then the evaluated image in loss mode
   if (!p->content_tap.empty()) FAV_TRY(run_pass(p, *pl, content, 0, st));
   FAV_TRY(run_pass(p, *pl, stylized, 1, st));
-  const size_t nc = p->content_tap.size(), nsty = p->style_tap.size();
-  for (size_t k = 0; k < nc; ++k) {  // nn.MSECriterion: mean over C*H*W
-    const PTap &a = pl->taps[1][p->content_tap[k]], &b = pl->taps[0][p->content_tap[k]];
-    percep_sqdiff_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(a.hi, a.lo, b.hi, b.lo, a.nkb * a.Cp, pl->red);
-    FAV_TRY(post_launch("percep_sqdiff"));
-    percep_sum_kernel<<<1, kRedThreads, 0, st>>>(pl->red, kRedBlocks, 1.0 / ((double)a.C * a.H * a.W), p->d_losses + k);
-    FAV_TRY(post_launch("percep_sum"));
+  FAV_TRY(launch_losses(p, *pl, st));
+  return finish_losses(p, *pl, st, content_loss, style_loss, nullptr);
+}
+
+int fav_percep_forward_backward(fav_percep_t *p, const float *content_pre, const float *input_pre, int H, int W, float *grad_input,
+                                double *content_loss, double *style_loss, double *layer_losses, void *stream) {
+  FAV_REQUIRE(p && input_pre && grad_input && content_loss && style_loss, "fav_percep_forward_backward: null argument");
+  FAV_REQUIRE(content_pre || p->content_tap.empty(), "fav_percep_forward_backward: the content layers need a content target");
+  FAV_REQUIRE(p->finalized, "fav_percep_forward_backward: call fav_percep_finalize first");
+  FAV_REQUIRE(p->has_target || p->style_tap.empty(), "fav_percep_forward_backward: set the style target first");
+  if (const int m = bwd_unsupported_module(p)) {
+    const PConv *pc = nullptr;
+    for (const PConv &c : p->convs)
+      if (c.module == m) pc = &c;
+    set_error("loss network module %d: convolution k%d stride %d pad %d: the backward pass runs stride-1 convolutions with pad "
+              "(k-1)/2 only", m, pc->k, pc->stride, pc->pad);
+    return FAV_ERR_UNSUPPORTED;
   }
-  for (size_t k = 0; k < nsty; ++k) {  // nn.MSECriterion over the C x C Gram matrix (or the C means)
-    const PTap &a = pl->taps[1][p->style_tap[k]];
-    FAV_TRY(aggregate(p, *pl, a, p->stat[k], st));
-    const int n = agg_len(p, a.C);
-    percep_vec_sqdiff_kernel<<<1, kRedThreads, 0, st>>>(p->stat[k], p->target[k], n, 1.0 / n, p->d_losses + nc + k);
-    FAV_TRY(post_launch("percep_vec_sqdiff"));
+  FAV_TRY(prepare_backward(p));
+  cudaStream_t st = (cudaStream_t)stream;
+  PPlan *pl;
+  FAV_TRY(build_pplan(p, H, W, &pl, true));
+  p->last_plan = pl;
+  FAV_TRY(check_cuda(cudaMemsetAsync(pl->overflow, 0, sizeof(int), st), "cudaMemsetAsync(overflow)"));
+  // PerceptualCriterion.lua:117-134 (setContentTarget, then the input in loss mode), then :158-161
+  if (!p->content_tap.empty()) FAV_TRY(run_pass(p, *pl, content_pre, 0, st, true));
+  FAV_TRY(run_pass(p, *pl, input_pre, 1, st, true));
+  FAV_TRY(launch_losses(p, *pl, st));
+  FAV_TRY(run_backward(p, *pl, grad_input, st));
+  return finish_losses(p, *pl, st, content_loss, style_loss, layer_losses);
+}
+
+int fav_pixel_loss_grad(const float *out2, const float *prev_warped_masked, const float *cert, int N, int H, int W, int type,
+                        float weight, float *grad_accum, double *loss, void *stream) {
+  FAV_REQUIRE(out2 && prev_warped_masked && cert && grad_accum && loss, "fav_pixel_loss_grad: null argument");
+  FAV_REQUIRE(N >= 1 && H >= 1 && W >= 1, "fav_pixel_loss_grad: bad size %dx%dx%d", N, H, W);
+  FAV_REQUIRE(type >= 0 && type <= 2, "fav_pixel_loss_grad: type must be 0 (L2), 1 (L1) or 2 (SmoothL1)");
+  FAV_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t HW = (int64_t)H * W, n = 3 * (int64_t)N * HW;
+  // the criterion's norm (THNN MSECriterion 2/n, AbsCriterion and SmoothL1Criterion 1/n), in fp32 as its `real`
+  const float norm = (float)((type == 0 ? 2.0 : 1.0) / (double)n);
+  double *part = nullptr;
+  FAV_TRY(check_cuda(cudaMallocAsync((void **)&part, (kRedBlocks + 1) * sizeof(double), st), "cudaMallocAsync(pixel loss)"));
+  fav_pixel_loss_grad_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(out2, prev_warped_masked, cert, HW, n, type, norm, weight, grad_accum, part);
+  int rc = post_launch("fav_pixel_loss_grad");
+  if (rc == FAV_OK) {
+    percep_sum_kernel<<<1, kRedThreads, 0, st>>>(part, kRedBlocks, (double)weight / (double)n, part + kRedBlocks);
+    rc = post_launch("percep_sum");
   }
-  std::vector<double> mse(nc + nsty + 1, 0.0);
-  FAV_TRY(check_cuda(cudaMemcpyAsync(mse.data(), p->d_losses, mse.size() * sizeof(double), cudaMemcpyDeviceToHost, st),
-                     "cudaMemcpyAsync(losses)"));
-  FAV_TRY(check_overflow(*pl, st));
-  // PerceptualCriterion.lua:141-152: total = sum over loss layers of strength * MSE, in layer order
-  double tc = 0.0, ts = 0.0;
-  for (size_t k = 0; k < nc; ++k) tc += p->content_w[k] * mse[k];
-  for (size_t k = 0; k < nsty; ++k) ts += p->style_w[k] * mse[nc + k];
-  *content_loss = tc;
-  *style_loss = ts;
-  return FAV_OK;
+  if (rc == FAV_OK)
+    rc = check_cuda(cudaMemcpyAsync(loss, part + kRedBlocks, sizeof(double), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync(pixel loss)");
+  const int rf = check_cuda(cudaFreeAsync(part, st), "cudaFreeAsync(pixel loss)");
+  if (rc == FAV_OK) rc = rf;
+  if (rc == FAV_OK) rc = check_cuda(cudaStreamSynchronize(st), "cudaStreamSynchronize(pixel loss)");
+  return rc;
+}
+
+int fav_tv_grad(const float *x, int N, int H, int W, float strength, float *grad_accum, void *stream) {
+  FAV_REQUIRE(x && grad_accum, "fav_tv_grad: null argument");
+  FAV_REQUIRE(N >= 1 && H >= 1 && W >= 1, "fav_tv_grad: bad size %dx%dx%d", N, H, W);
+  FAV_TRY(require_device());
+  const int64_t planes = 3 * (int64_t)N, total = planes * H * W;
+  fav_tv_grad_kernel<<<(unsigned)ceil_div64(total, 256), 256, 0, (cudaStream_t)stream>>>(x, planes, H, W, strength, grad_accum);
+  return post_launch("fav_tv_grad");
 }
 
 int fav_percep_layer_output(fav_percep_t *p, int pass, int index, float *out, int *C, int *Hl, int *Wl, void *stream) {

@@ -96,6 +96,10 @@ SIGNATURES = {
     "fav_percep_layer_output": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                           C.POINTER(C.c_int), _fp]),
     "fav_percep_style_stat": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), _fp]),
+    "fav_percep_forward_backward": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, _fp, C.POINTER(C.c_double),
+                                              C.POINTER(C.c_double), C.POINTER(C.c_double), _fp]),
+    "fav_pixel_loss_grad": (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _fp, C.POINTER(C.c_double), _fp]),
+    "fav_tv_grad": (C.c_int, [_fp, C.c_int, C.c_int, C.c_int, C.c_float, _fp, _fp]),
     "fav_debug_set_trace": (C.c_int, [_fp, C.c_size_t]),
     "fav_debug_trace_words": (C.c_size_t, []),
     "fav_run_image": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, _fp, _fp]),

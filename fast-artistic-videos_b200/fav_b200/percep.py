@@ -160,6 +160,65 @@ class PerceptualCriterion:
         _lib.check(_lib.lib.fav_percep_layer_output(self._h, pass_, index, _lib.dptr(out), None, None, None, _lib.stream_ptr()))
         return out
 
+    def forward(self, input: torch.Tensor, target) -> float:
+        """percep_crit:forward(input, {content_target=...}) (PerceptualCriterion.lua:117-155, train_video.lua:343-344).
+
+        input and target['content_target']: [N,3,H,W] (or [3,H,W]) in NET space, BGR 255 x - mean, as the training script
+        feeds them; the style target is the one set_style_target captured.  Sets total_content_loss, total_style_loss,
+        content_losses and style_losses (strength * MSE per layer) and returns their sum.  The gradient is computed in the same
+        pass and returned by backward().  A batch is one call per image, scaled by 1/N: MSE over N*C*H*W for the content layers
+        and over the N*C*C expanded target for the style layers (StyleLoss.lua:39-50) is the mean of the per-image losses."""
+        x = self._batch(input)
+        ct = target.get("content_target") if isinstance(target, dict) else target
+        if isinstance(target, dict) and target.get("style_target") is not None:
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, "forward: set the style target with set_style_target (an RGB image)")
+        if ct is None and self.content_layers:
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, "forward: the content layers need target['content_target']")
+        ct = self._batch(ct) if ct is not None else None
+        if ct is not None and ct.shape != x.shape:
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, f"forward: input {tuple(x.shape)} and content target {tuple(ct.shape)} differ")
+        N, _, H, W = x.shape
+        nc, ns = len(self.content_layers), len(self.style_layers)
+        grad = torch.empty_like(x)
+        per = np.zeros(nc + ns)
+        tc = ts = 0.0
+        for n in range(N):
+            cl, sl, lay = C.c_double(), C.c_double(), (C.c_double * max(1, nc + ns))()
+            _lib.check(_lib.lib.fav_percep_forward_backward(self._h, _lib.dptr(ct[n]) if ct is not None else None, _lib.dptr(x[n]), H, W,
+                                                            _lib.dptr(grad[n]), C.byref(cl), C.byref(sl), lay, _lib.stream_ptr()))
+            tc += cl.value
+            ts += sl.value
+            per += np.asarray(lay[:nc + ns])
+        if N > 1:
+            grad.mul_(1.0 / N)
+        self.total_content_loss, self.total_style_loss = tc / N, ts / N
+        self.content_losses = [float(v) / N for v in per[:nc]]
+        self.style_losses = [float(v) / N for v in per[nc:]]
+        self.output = self.total_style_loss + self.total_content_loss
+        self.gradInput = grad
+        self._fb_args = (input, target)
+        return self.output
+
+    updateOutput = forward
+
+    def backward(self, input: torch.Tensor, target) -> torch.Tensor:
+        """percep_crit:backward(input, target) (PerceptualCriterion.lua:158-161): d output / d input, [N,3,H,W] net space."""
+        args = getattr(self, "_fb_args", None)
+        if args is None or args[0] is not input or args[1] is not target:
+            self.forward(input, target)
+        return self.gradInput
+
+    updateGradInput = backward
+
+    @staticmethod
+    def _batch(img: torch.Tensor) -> torch.Tensor:
+        t = img.detach().to(device="cuda", dtype=torch.float32)
+        if t.dim() == 3:
+            t = t[None]
+        if t.dim() != 4 or t.shape[1] != 3:
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, f"expected [N,3,H,W] images, got {tuple(img.shape)}")
+        return t.contiguous()
+
     def style_stat(self, which: int, k: int) -> torch.Tensor:
         """Gram matrix [C,C] (or the C means) of style layer k: which 0 = style target, 1 = last evaluated image."""
         n = C.c_int()
@@ -170,6 +229,45 @@ class PerceptualCriterion:
             c = int(round(n.value ** 0.5))
             out = out.reshape(c, c)
         return out
+
+
+PIXEL_LOSS_TYPES = {"L2": 0, "L1": 1, "SmoothL1": 2}
+
+
+def _nchw3(t: torch.Tensor, what: str) -> torch.Tensor:
+    if t.device.type != "cuda" or t.dtype != torch.float32 or not t.is_contiguous() or t.dim() != 4 or t.shape[1] != 3:
+        raise _lib.FavError(_lib.FAV_ERR_INVALID, f"{what}: expected a contiguous CUDA float32 [N,3,H,W] tensor, got "
+                                                  f"{tuple(t.shape)} {t.dtype} on {t.device}")
+    return t
+
+
+def pixel_loss_grad(out2: torch.Tensor, prev_warped_masked: torch.Tensor, cert: torch.Tensor, loss_type: str, weight: float,
+                    grad_accum: torch.Tensor) -> float:
+    """pixel_crit:forward / backward(out2 .* cert, out1_warped_masked) scaled by -pixel_loss_weight (train_video.lua:117-126,
+    354-366): returns weight * loss and adds weight * d loss / d (out2 .* cert) to grad_accum in place, NOT multiplied by the
+    certainty (the script adds the criterion's gradInput as it is).  out2, prev_warped_masked, grad_accum [N,3,H,W];
+    cert [N,1,H,W]."""
+    if loss_type not in PIXEL_LOSS_TYPES:
+        raise ValueError(f"pixel loss type {loss_type!r}: L2, L1 or SmoothL1")
+    N, _, H, W = _nchw3(out2, "out2").shape
+    _nchw3(grad_accum, "grad_accum")
+    prev = _nchw3(prev_warped_masked, "prev_warped_masked")
+    if prev.shape != out2.shape or grad_accum.shape != out2.shape or tuple(cert.shape) != (N, 1, H, W):
+        raise _lib.FavError(_lib.FAV_ERR_INVALID, "pixel_loss_grad: shape mismatch")
+    c = cert.detach().to(device="cuda", dtype=torch.float32).contiguous()
+    loss = C.c_double()
+    _lib.check(_lib.lib.fav_pixel_loss_grad(_lib.dptr(out2), _lib.dptr(prev), _lib.dptr(c), N, H, W, PIXEL_LOSS_TYPES[loss_type],
+                                            float(weight), _lib.dptr(grad_accum), C.byref(loss), _lib.stream_ptr()))
+    return loss.value
+
+
+def tv_grad(x: torch.Tensor, strength: float, grad_accum: torch.Tensor) -> torch.Tensor:
+    """nn.TotalVariation(strength):updateGradInput(x, grad_accum) (TotalVariation.lua:19-35), in place on grad_accum."""
+    N, _, H, W = _nchw3(x, "x").shape
+    if _nchw3(grad_accum, "grad_accum").shape != x.shape:
+        raise _lib.FavError(_lib.FAV_ERR_INVALID, "tv_grad: shape mismatch")
+    _lib.check(_lib.lib.fav_tv_grad(_lib.dptr(x), N, H, W, float(strength), _lib.dptr(grad_accum), _lib.stream_ptr()))
+    return grad_accum
 
 
 def scale_style_image(img: torch.Tensor, size: int) -> torch.Tensor:

@@ -272,6 +272,25 @@ FAV_API int fav_percep_layer_output(fav_percep_t *p, int pass, int index, float 
 /* tests: the aggregate (StyleLoss.lua:40-43) of style layer k (0-based position in the style layer list) as DEVICE
  * doubles: Gram matrix C*C (GramMatrix.lua:31-53) or C means; which 0 = style target, 1 = last evaluated image. */
 FAV_API int fav_percep_style_stat(fav_percep_t *p, int which, int k, double *out, int *n, void *stream);
+/* percep_crit:forward(input, {content_target=...}) then percep_crit:backward(input, target)   train_video.lua:343-345,
+ * PerceptualCriterion.lua:117-161, ContentLoss.lua:50-59, StyleLoss.lua:57-67, GramMatrix.lua:54-78.
+ * content_pre, input_pre [3,H,W] device fp32 in NET space (BGR, 255 x - mean; content_pre may be NULL without content layers);
+ * writes grad_input [3,H,W] (d total / d input_pre), the two totals and, if layer_losses is not NULL, strength * MSE of every
+ * loss layer (content layers, then style layers) through HOST doubles (synchronises `stream`).  Every convolution up to the
+ * deepest loss layer must be stride 1 with pad (k-1)/2 (FAV_ERR_UNSUPPORTED naming the module otherwise, before any device
+ * work).  The first call at a size keeps every convolution's fp32 output (about 1.1 GB at 1280x720 to relu4_3). */
+FAV_API int fav_percep_forward_backward(fav_percep_t *p, const float *content_pre, const float *input_pre, int H, int W,
+                                        float *grad_input, double *content_loss, double *style_loss, double *layer_losses,
+                                        void *stream);
+/* pixel_crit:forward / backward(out2 .* cert, out1_warped_masked)   train_video.lua:117-126,354-366
+ * out2, prev_warped_masked [N,3,H,W], cert [N,1,H,W] device fp32; type 0 L2 (MSECriterion), 1 L1 (AbsCriterion), 2 SmoothL1;
+ * sizeAverage.  grad_accum [N,3,H,W] += weight * d loss / d (out2 .* cert) -- NOT multiplied by cert, as train_video.lua:357-364
+ * adds it; *loss = weight * loss (HOST double, synchronises `stream`). */
+FAV_API int fav_pixel_loss_grad(const float *out2, const float *prev_warped_masked, const float *cert, int N, int H, int W,
+                                int type, float weight, float *grad_accum, double *loss, void *stream);
+/* nn.TotalVariation:updateGradInput with gradOutput = grad_accum   TotalVariation.lua:19-35
+ * x, grad_accum [N,3,H,W] device fp32: grad_accum += strength * (TV gradient over the {1,-2} ranges). */
+FAV_API int fav_tv_grad(const float *x, int N, int H, int W, float strength, float *grad_accum, void *stream);
 
 /* diagnostics: per-CTA timeline of the following tensor-core convolution launches (entry / set-up /
  * exit clock64 marks, 64 u64 words per CTA, launches appended) into a caller-owned DEVICE buffer; NULL = off. */
