@@ -23,7 +23,7 @@ struct KStep {
   uint16_t lbo16;
 };
 
-// tensor-core (wgmma) implicit-GEMM job (one convolution, or one sub-pixel phase of a transposed convolution)
+// tensor-core (wgmma) implicit-GEMM job (one convolution, or one or several stacked sub-pixel phases of a transposed convolution)
 struct ConvJob {
   // input operand (hi/lo fp16 planes), addressed in 16-byte units
   const uint4 *a_hi, *a_lo;
@@ -92,6 +92,9 @@ struct ConvJob {
   float *raw;
   int raw_Cq, raw_Wp;
   int oy_mul, oy_off, ox_mul, ox_off;
+  // stacked sub-pixel phases of a stride-2 transposed conv (plan_phase_stack): accumulator column n = s * Cout + c is channel
+  // c of phase s, placed at raw(y*oy_mul + st_oy[s], x*ox_mul + st_ox[s]) (stack_epi_addr).  0: one phase per job
+  int nstack, st_oy[4], st_ox[4];
   // final layer: Tanh -> MulConstant(tanh_c) [-> deprocess] written as fp32 NCHW [3][outH][outW]
   int final_mode;  // 0 = raw, 1 = net space, 2 = fused vgg.deprocess
   float *out3;
@@ -146,6 +149,26 @@ __host__ __device__ inline bool opnd_epi_addr(const ConvJob &j, int tile, int t,
                                               bool batch = true) {
   return opnd_epi_addr(j, tile_at(j, tile, batch), t, i, h, dst4, skip4);
 }
+
+// Stacked-phase epilogue addressing (ConvJob::nstack > 0), shared by conv_tc_kernel and its CPU emulator
+// (tests/emu/phase_stack_emu.cu).  Consumer thread t holds the accumulator pair of columns n, n + 1 (n = 8i + 2 (t % 4)) of tile
+// pixel r0 + 8h, as in opnd_epi_addr.  They are channels c, c + 1 of phase s = n / Cout (Cout % 8 == 0, so s = 8i / Cout and
+// both columns lie in one phase).  Returns false when the pixel lies outside the job's grid (no store); else the float offset
+// of the pair in the image's raw output.
+__host__ __device__ inline bool stack_epi_addr(const ConvJob &j, int y, int x0, int t, int i, int h, int64_t &raw_off) {
+  const int s = 8 * i / j.Cout, c = 8 * i + 2 * (t & 3) - s * j.Cout;
+  const int x = x0 + (t >> 7) * 64 + ((t >> 5) & 3) * 16 + ((t & 31) >> 2) + 8 * h;
+  if (x >= j.Wo || y >= j.Ho || s >= j.nstack) return false;
+  const int yo = y * j.oy_mul + j.st_oy[s], xo = x * j.ox_mul + j.st_ox[s];
+  raw_off = (((int64_t)yo * j.raw_Cq + (c >> 2)) * j.raw_Wp + xo) * 4 + (c & 3);
+  return true;
+}
+// Fused statistics: the per-warp partial sums are kept per accumulator column, and column n flushes into channel
+// stats_channel(n) of the job's [sum][sum of squares] array (tc_flush_stats; columns >= stats_columns hold padding).  A stacked
+// job thus sends each phase's partial sums out separately, the same float partials the one-job-per-phase plan sends, so the
+// double totals -- and the normalised layer -- are the per-phase plan's.
+__host__ __device__ inline int stats_columns(const ConvJob &j) { return j.nstack ? j.nstack * j.Cout : j.Cout; }
+__host__ __device__ inline int stats_channel(const ConvJob &j, int n) { return j.nstack ? n % j.Cout : n; }
 
 // Norm-on-load addressing, shared by the producer warps of conv_tc_kernel and their CPU emulator (tests/emu/nl_geom_emu.cu).
 // The producer stages, for every patch pixel, the value the bulk copies would read from the operand that in_apply writes:

@@ -32,6 +32,9 @@ struct ConvPhase {
   int nchunks = 1, spc = 1;
   int rf_R = 0, rf_rps = 0;                    // row-fold: output rows per unit, patch rows per stage (0 = off)
   int pf = 0;                                  // phase-fold (transposed conv): see conv.cuh
+  // stacked job (plan_phase_stack): nstack sub-pixel phases along N, phase s at output offset (stack_oy[s], stack_ox[s]) in
+  // columns [s Cout, (s + 1) Cout); its taps are the union of theirs (ky / kx unused).  0: an ordinary phase
+  int nstack = 0, stack_oy[4] = {0, 0, 0, 0}, stack_ox[4] = {0, 0, 0, 0};
   std::vector<KStep> steps;                    // per group
   std::vector<std::vector<Unit>> units;        // [group][step*2 + u]
   float *d_w_simt = nullptr;
@@ -59,6 +62,10 @@ struct ConvDef {
   // Cout > kMaxNBlock (stylization net): the ConvDef of each N block (plan_conv_nblocks); the tensor-core jobs come from
   // these, the CUDA-core comparator keeps the whole convolution's phases.  Empty: one job per phase of this ConvDef.
   std::vector<ConvDef> nblock;
+  // stride-2 transposed conv with 2 Cout <= 128 (plan_phase_stack): the tensor-core jobs with the sub-pixel phases stacked
+  // along N, and their bias (the layer's, once per stacked phase).  Empty: one job per phase.
+  std::vector<ConvPhase> stack;
+  float *d_stack_bias = nullptr;
   float *d_bias = nullptr;
   float *d_scale = nullptr;  // batch-normalized nets: the per-channel BN scale the operand epilogue applies (Npad floats)
   int pw = -1, pb = -1;  // param indices
@@ -95,7 +102,7 @@ static inline int build_phase_tables(const ConvDef &c, ConvPhase &ph) {
     return -1;
   };
   const int nrows = (int)ph.rows.size();
-  ph.Npad = c.Npad;
+  ph.Npad = ph.nstack ? round_up(ph.nstack * c.cout, 16) : c.Npad;
   const bool xfold = !c.raw_out && !c.transposed && c.in_stride == 1 && c.k >= 5 && c.cout <= 4 && c.Cb % 2 == 0 && c.pad == (c.k - 1) / 2;
   if (xfold) {
     ph.kind = 3; ph.Npad = round_up(c.k * c.cout, 16);
@@ -433,6 +440,41 @@ static inline int plan_conv_nblocks(ConvDef &c) {
   return FAV_OK;
 }
 
+// ---- stacked sub-pixel phases: the phases of a stride-2 transposed conv share their input pixels, only the weights and the
+// output placement differ.  So as many phases as fit N <= 128 run as one stride-1 conv over the input grid, phase s in columns
+// [s Cout, (s + 1) Cout): all four when 4 Cout <= 128, else the two column phases b = 0, 1 of each row phase a.  The job's taps
+// are the union of its phases' taps; where a tap does not feed phase s its weights are zero (extra MMA work, the useful FLOPs
+// are unchanged).  Cout % 8 == 0 keeps each epilogue column pair inside one phase (stack_epi_addr).  c.phases stay as they
+// are for the CUDA-core comparator and for batch-normalized nets, whose operand epilogue runs one phase per job.
+static inline int plan_phase_stack(ConvDef &c) {
+  c.stack.clear();
+  if (!c.transposed || c.stride != 2 || c.cout % 8 || 2 * c.cout > kMaxNBlock) return FAV_OK;
+  const int per_job = 4 * c.cout <= kMaxNBlock ? 4 : 2;  // c.phases: (a, b) = (0,0), (0,1), (1,0), (1,1)
+  for (int p0 = 0; p0 < 4; p0 += per_job) {
+    ConvPhase ph;
+    ph.nstack = per_job;
+    for (int s = 0; s < per_job; ++s) {
+      const ConvPhase &p = c.phases[p0 + s];
+      ph.stack_oy[s] = p.oy_off; ph.stack_ox[s] = p.ox_off;
+      for (const ConvTap &t : p.taps) {
+        bool have = false;
+        for (const ConvTap &u : ph.taps) have = have || (u.dy == t.dy && u.dx == t.dx);
+        if (!have) ph.taps.push_back(ConvTap{t.dy, t.dx, -1, -1});
+      }
+    }
+    FAV_TRY(build_phase_tables(c, ph));
+    c.stack.push_back(std::move(ph));
+  }
+  return FAV_OK;
+}
+// the bias of a stacked job (Npad floats): column s * Cout + co holds the layer's bias of channel co
+static inline std::vector<float> stack_bias(const ConvDef &c, const std::vector<float> &b) {
+  const ConvPhase &ph = c.stack[0];
+  std::vector<float> sb(ph.Npad, 0.f);
+  for (int n = 0; n < ph.nstack * c.cout; ++n) sb[n] = b[n % c.cout];
+  return sb;
+}
+
 // packed tcgen05 weights of one phase: [group][chunk][hi|lo][step][k8 half][Npad][8] fp16 (as uint16 bit patterns)
 static inline std::vector<uint16_t> pack_phase_weights(const ConvDef &c, const ConvPhase &ph, const std::vector<float> &w) {
   if (ph.rf_R) {
@@ -478,6 +520,11 @@ static inline std::vector<uint16_t> pack_phase_weights(const ConvDef &c, const C
                 if (ph.kind == 3) {  // n = kx * Cout + co, unit.tap = ky
                   int kx = n / c.cout, co = n % c.cout;
                   v = kx < c.k ? weight_at(c, w, co, un.cb * 8 + i, un.tap, kx) : 0.f;
+                } else if (ph.nstack) {  // n = s * Cout + co; tap (dy, dx) of phase (a, b) is filter tap (a + pad - 2 dy, b + pad - 2 dx)
+                  const int s = n / c.cout, co = n % c.cout;
+                  const int ky = s < ph.nstack ? ph.stack_oy[s] + c.pad - c.stride * ph.taps[un.tap].dy : -1;
+                  const int kx = s < ph.nstack ? ph.stack_ox[s] + c.pad - c.stride * ph.taps[un.tap].dx : -1;
+                  v = ky >= 0 && ky < c.k && kx >= 0 && kx < c.k ? weight_at(c, w, co, un.cb * 8 + i, ky, kx) : 0.f;
                 } else {
                   v = weight_at(c, w, n, un.cb * 8 + i, ph.taps[un.tap].ky, ph.taps[un.tap].kx);
                 }
@@ -586,6 +633,8 @@ static inline int fill_conv_job(const ConvDef &c, const ConvPhase &ph, const Ope
     }
   }
   j.oy_mul = c.out_mul; j.ox_mul = c.out_mul; j.oy_off = ph.oy_off; j.ox_off = ph.ox_off;
+  j.nstack = ph.nstack;
+  for (int s = 0; s < ph.nstack; ++s) { j.st_oy[s] = ph.stack_oy[s]; j.st_ox[s] = ph.stack_ox[s]; }
   // every bulk copy must stay inside the operand allocation
   int64_t max_row = (int64_t)j.row_mul * (ceil_div(pHo, j.mt) * j.mt - 1) + in.padT + ph.rows.back();
   if (ph.rf_R) max_row = (int64_t)(ceil_div(pHo, j.mt) - 1) * j.mt + in.padT + ph.rows[0] + j.rf_total_rows - 1;

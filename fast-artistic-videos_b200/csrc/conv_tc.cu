@@ -23,7 +23,8 @@
 //   warp  9     A producer (bulk copies of the patch, all lanes issue)
 //   warps 9-15  norm-on-load jobs: patch producers (raw fp32 -> InstanceNorm + ReLU -> fp16 hi/lo staged for the MMA,
 //               replacing a separate in_apply pass)
-// Plans per layer family (conv_plan.hpp): generic, stride-2 parity split, tap pairing (Cin = 8), x-fold.
+// Plans per layer family (conv_plan.hpp): generic, stride-2 parity split, tap pairing (Cin = 8), x-fold; the sub-pixel phases
+// of a stride-2 transposed conv stacked along N (plan_phase_stack).
 // Pipelines: A stages and weight slots with full/empty mbarriers; each consumer warpgroup releases a slot once its
 // wgmmas that read it have completed.
 #include <atomic>
@@ -66,25 +67,43 @@ __device__ __forceinline__ void trace_put(const ConvJob &job, int word, long lon
   if (job.trace) job.trace[(size_t)blockIdx.x * kTraceWords + word] = (unsigned long long)v;
 }
 
-// fused statistics of image b: the 8 warps' partial sums added in a FIXED order (deterministic per CTA: the tile -> CTA assignment
-// is static), then one double atomic per channel and quantity per CTA.  reset: the partials are zeroed for the next image (thread
-// ch clears the column it has just read; the closing barrier keeps the next tile's writers behind it).
+// fused statistics of image b: the 8 warps' partial sums of each accumulator column added in a FIXED order (deterministic per
+// CTA: the tile -> CTA assignment is static), then one double atomic per column and quantity per CTA into its channel
+// (stats_channel: a stacked job's phases add into the same channels one after the other).  reset: the partials are zeroed for
+// the next image (thread ch clears the column it has just read; the closing barrier keeps the next tile's writers behind it).
 __device__ __forceinline__ void tc_flush_stats(const ConvJob &job, float *slot, int b, bool reset) {
   asm volatile("bar.sync 1, 256;" ::: "memory");
-  const int ch = threadIdx.x;
-  if (ch < job.Cout) {
+  const int ch = threadIdx.x;  // accumulator column
+  if (ch < stats_columns(job)) {
     float ssum = 0.f, qsum = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) { ssum += slot[w * 256 + ch]; qsum += slot[w * 256 + 128 + ch]; }
     double *st = job.stats + b * job.stats_img;
-    atomicAdd(st + ch, (double)ssum);
-    atomicAdd(st + job.stats_pitch + ch, (double)qsum);
+    const int c = stats_channel(job, ch);
+    atomicAdd(st + c, (double)ssum);
+    atomicAdd(st + job.stats_pitch + c, (double)qsum);
   }
   if (reset) {
     if (ch < 128)
 #pragma unroll
       for (int w = 0; w < 8; ++w) { slot[w * 256 + ch] = 0.f; slot[w * 256 + 128 + ch] = 0.f; }
     asm volatile("bar.sync 1, 256;" ::: "memory");
+  }
+}
+
+// fused statistics of one column pair: v = {pixel r0: c, c + 1, pixel r0 + 8: c, c + 1} (zero where not stored) summed over the
+// warp's 16 pixels (the 8 lanes that share lane % 4), then added into the warp's slot of accumulator columns c, c + 1 by one
+// writer per (warp, column): deterministic
+__device__ __forceinline__ void tc_stats_add(float *slot, int warp, int lane, int c, const float v[4]) {
+  float s0 = v[0] + v[2], s1 = v[1] + v[3], t0 = v[0] * v[0] + v[2] * v[2], t1 = v[1] * v[1] + v[3] * v[3];
+#pragma unroll
+  for (int m = 4; m < 32; m <<= 1) {
+    s0 += __shfl_xor_sync(0xffffffffu, s0, m); s1 += __shfl_xor_sync(0xffffffffu, s1, m);
+    t0 += __shfl_xor_sync(0xffffffffu, t0, m); t1 += __shfl_xor_sync(0xffffffffu, t1, m);
+  }
+  if (lane < 4) {
+    float *sl = slot + warp * 256;
+    sl[c] += s0; sl[c + 1] += s1; sl[128 + c] += t0; sl[128 + c + 1] += t1;
   }
 }
 
@@ -209,6 +228,30 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
           }
         continue;
       }
+      if (!OPND && job.nstack) {
+        // stacked sub-pixel phases: column pair n of phase s = n / Cout goes to that phase's output pixel (stack_epi_addr); its
+        // statistics stay in column n until tc_flush_stats
+        const bool stats = job.stats && !(job.dbg & 64);
+        float *raw = job.raw + img.raw;
+  #pragma unroll
+        for (int i = 0; i < NJ; ++i) {
+          const int n = 8 * i + q2;
+          const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + n));  // the bias of each stacked phase
+          float v[4];
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            int64_t o = 0;
+            v[2 * h] = acc[4 * i + 2 * h] + b.x;
+            v[2 * h + 1] = acc[4 * i + 2 * h + 1] + b.y;
+            if (stack_epi_addr(job, y, x0, threadIdx.x, i, h, o) && !(job.dbg & 1))
+              *reinterpret_cast<float2 *>(raw + o) = make_float2(v[2 * h], v[2 * h + 1]);
+            else
+              v[2 * h] = v[2 * h + 1] = 0.f;
+          }
+          if (stats) tc_stats_add(slot, warp, lane, n, v);
+        }
+        continue;
+      }
       if constexpr (OPND) {
         // the two channels c, c + 1 of each of the thread's two pixels: BN scale and bias (+ReLU) (+skip) -> fp16 hi / lo pair, one 4-byte store
         // per plane; the 4 lanes of a quad fill one 16-byte (pixel, channel block) cell.  No statistics, no atomics.
@@ -257,19 +300,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
                 make_float2(v[2 * h], v[2 * h + 1]);
           if (!valid[h]) v[2 * h] = v[2 * h + 1] = 0.f;
         }
-        if (stats) {
-          // per-channel sums over the warp's 16 pixels: reduce over the 8 lanes that share lane % 4
-          float s0 = v[0] + v[2], s1 = v[1] + v[3], t0 = v[0] * v[0] + v[2] * v[2], t1 = v[1] * v[1] + v[3] * v[3];
-  #pragma unroll
-          for (int m = 4; m < 32; m <<= 1) {
-            s0 += __shfl_xor_sync(0xffffffffu, s0, m); s1 += __shfl_xor_sync(0xffffffffu, s1, m);
-            t0 += __shfl_xor_sync(0xffffffffu, t0, m); t1 += __shfl_xor_sync(0xffffffffu, t1, m);
-          }
-          if (lane < 4) {  // one writer per (warp, channel): deterministic
-            float *sl = slot + warp * 256;
-            sl[c] += s0; sl[c + 1] += s1; sl[128 + c] += t0; sl[128 + c + 1] += t1;
-          }
-        }
+        if (stats) tc_stats_add(slot, warp, lane, c, v);
       }
     }
     if (!OPND && job.stats) tc_flush_stats(job, slot, img.b, tile < total);  // an operand epilogue has no statistics

@@ -245,6 +245,14 @@ static int pack_conv_weights(fav_net *net, ConvDef &c, const std::vector<float> 
     FAV_TRY(dev_upload(net, ws, &ph.d_w_simt));
   }
   if (c.nblock.empty()) FAV_TRY(pack_tc_weights(net, c, w));
+  if (!c.stack.empty()) {  // stacked sub-pixel phases: column s * Cout + co holds channel co of phase s
+    FAV_TRY(dev_upload(net, stack_bias(c, b), &c.d_stack_bias));
+    for (ConvPhase &ph : c.stack) {
+      uint16_t *d = nullptr;
+      FAV_TRY(dev_upload(net, pack_phase_weights(c, ph, w), &d));
+      ph.d_b_tc = reinterpret_cast<uint4 *>(d);
+    }
+  }
   if (c.has_fold) {  // transposed conv: one tcgen05 job for all four sub-pixel phases
     std::vector<uint16_t> pk = pack_phase_fold(c, c.fold, w);
     uint16_t *d = nullptr;
@@ -324,18 +332,20 @@ static int make_operand(Plan &pl, int C, int H, int W, const ConvDef *consumer, 
   return FAV_OK;
 }
 
-// tensor-core jobs of c (one per phase, per N block when Cout > kMaxNBlock) and CUDA-core comparator jobs (one per phase);
-// stats: the [sum][sum of squares] slots of c's output for the fused InstanceNorm statistics, or null; epi (batch-normalized
-// nets): the operand step whose ReLU / skip / packing the tensor-core epilogue performs (set_opnd_epilogue), or null
+// tensor-core jobs of c (one per phase, per N block when Cout > kMaxNBlock, or the stacked-phase jobs of plan_phase_stack) and
+// CUDA-core comparator jobs (one per phase); stats: the [sum][sum of squares] slots of c's output for the fused InstanceNorm
+// statistics, or null; epi (batch-normalized nets): the operand step whose ReLU / skip / packing the tensor-core epilogue
+// performs (set_opnd_epilogue), or null.  FAV_NO_STACK keeps one job per phase, so one process can compare the two plans.
 static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &c, bool last, float *out3, double *stats,
                            const PlanStep *epi = nullptr) {
   const Operand &in = pl.ops[st.src];
   const int nb = c.nblock.empty() ? 1 : (int)c.nblock.size();
+  const bool stack = !c.stack.empty() && !epi && !getenv("FAV_NO_STACK");
   for (int b = 0; b < nb; ++b) {
     const ConvDef &cd = c.nblock.empty() ? c : c.nblock[b];
     float *raw = st.raw.p + conv_nblock_raw_offset(b, st.raw.Wp);
     bool fold_done = false;
-    for (const ConvPhase &ph : cd.phases) {
+    for (const ConvPhase &ph : stack ? c.stack : cd.phases) {
       const bool use_fold = cd.has_fold && !getenv("FAV_NO_FOLD");
       ConvJob j;
       if (use_fold) {
@@ -355,7 +365,7 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
       } else {
         FAV_TRY(fill_conv_job(cd, ph, in, j));
         set_conv_batch(j, pl.B, st.raw.img, 3ll * pl.H * pl.W, pl.stats_img);
-        j.b = ph.d_b_tc; j.bias = cd.d_bias;
+        j.b = ph.d_b_tc; j.bias = stack ? c.d_stack_bias : cd.d_bias;
         j.raw = raw; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
         j.final_mode = last ? 1 : 0; j.out3 = out3; j.tanh_c = net->tanh_c;
         conv_nblock_stats(j, stats, c.cout, b);
@@ -865,7 +875,10 @@ int fav_net_finalize(fav_net_t *net) {
   FAV_TRY(fold_batch_norms(net, cw, cb, cs));
   // K-step tables (N blocks for Cout > 128) of every convolution, before any device work: a layer the tensor-core path
   // cannot run is refused here, by name, rather than at the first forward
-  for (ConvDef &c : net->convs) FAV_TRY(plan_conv_nblocks(c));
+  for (ConvDef &c : net->convs) {
+    FAV_TRY(plan_conv_nblocks(c));
+    if (!net->bn) FAV_TRY(plan_phase_stack(c));  // a batch-normalized net's operand epilogue runs one phase per job
+  }
   FAV_TRY(require_device());
   cudaDeviceProp prop;
   FAV_TRY(check_cuda(cudaGetDevice(&net->device), "cudaGetDevice"));
