@@ -335,6 +335,16 @@ __global__ void __launch_bounds__(256) percep_unpack_tap_kernel(const uint16_t *
   out[(int64_t)c * P + p] = __half2float(__ushort_as_half(hi[o])) + __half2float(__ushort_as_half(lo[o]));
 }
 
+// raw conv output (layout [H][Cq][Wp][4]) -> fp32 NCHW [C][H][W] (tests, fav_percep_conv_output)
+__global__ void __launch_bounds__(256) percep_unpack_raw_kernel(const float *__restrict__ raw, int Cq, int Wp, int C, int H, int W,
+                                                                float *__restrict__ out) {
+  const int64_t p = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  const int c = blockIdx.y;
+  if (p >= (int64_t)H * W) return;
+  const int y = (int)(p / W), x = (int)(p - (int64_t)y * W);
+  out[(int64_t)c * H * W + p] = raw[(((int64_t)y * Cq + (c >> 2)) * Wp + x) * 4 + (c & 3)];
+}
+
 // ---- backward (fav_percep_forward_backward) ---------------------------------------------------------------------------
 // The input gradient of a stride-1 convolution with pad (k-1)/2 is the same convolution geometry over the output gradient, with
 // the filters transposed and flipped: it runs on conv_tc_kernel like the forward.  Its operand is the fp16 hi/lo pair, whose
@@ -745,6 +755,7 @@ struct fav_percep {
   std::map<std::pair<int, int>, std::unique_ptr<PPlan>> plans;
   std::map<std::pair<int, int>, std::unique_ptr<PPlan>> bplans;  // fav_percep_forward_backward: raw outputs kept
   PPlan *last_plan = nullptr;
+  bool last_backward = false;     // last_plan is a backward plan (fav_percep_conv_output)
   std::vector<double *> target, stat;  // per style layer: aggregate of the style image / of the last evaluated image
   double *d_losses = nullptr;          // [n_content + n_style]
   std::vector<void *> allocs;
@@ -1058,6 +1069,18 @@ static int bwd_unsupported_module(const fav_percep *P) {
   return 0;
 }
 
+// host-only: the first stage with more gradient terms than percep_bwd_stage_kernel takes (its loss layers, plus the next stage's
+// input gradient), as the module index of its convolution; 0 if none
+static int bwd_crowded_stage(const fav_percep *P) {
+  const int ns = (int)P->convs.size();
+  for (int s = 0; s < ns; ++s) {
+    int nt = s + 1 < ns;
+    for (const PTapSpec &ts : P->taps) nt += ts.stage == s;
+    if (nt > kMaxStageTerms) return P->convs[s].module;
+  }
+  return 0;
+}
+
 // the input-gradient convolutions: W'[ci][co][ky][kx] = W[co][ci][k-1-ky][k-1-kx], a [cin][cout][k][k] tensor read as the
 // weights of a cout -> cin convolution, packed per 128-channel N block of cin like the forward's
 static int prepare_backward(fav_percep *P) {
@@ -1145,10 +1168,6 @@ static int run_backward(fav_percep *P, PPlan &pl, float *grad_input, cudaStream_
     for (size_t t = 0; t < P->taps.size(); ++t) {
       const PTapSpec &ts = P->taps[t];
       if (ts.stage != s) continue;
-      if (bs.nt == kMaxStageTerms) {
-        set_error("loss network: more than %d loss layers between two convolutions", kMaxStageTerms - 1);
-        return FAV_ERR_UNSUPPORTED;
-      }
       const PTap &tp = pl.taps[1][t];
       bs.t[bs.nt++] = BwdTerm{pl.tgrad[t], tp.H, tp.W, ts.relu, ts.pool.on};
       if (ts.pool.on) bs.pool = ts.pool;
@@ -1361,6 +1380,7 @@ int fav_percep_set_style_target(fav_percep_t *p, const float *rgb, int H, int W,
   PPlan *pl;
   FAV_TRY(build_pplan(p, H, W, &pl));
   p->last_plan = pl;
+  p->last_backward = false;
   FAV_TRY(check_cuda(cudaMemsetAsync(pl->overflow, 0, sizeof(int), st), "cudaMemsetAsync(overflow)"));
   FAV_TRY(run_pass(p, *pl, rgb, 1, st));
   for (size_t k = 0; k < p->style_tap.size(); ++k) FAV_TRY(aggregate(p, *pl, pl->taps[1][p->style_tap[k]], p->target[k], st));
@@ -1378,6 +1398,7 @@ int fav_percep_evaluate(fav_percep_t *p, const float *content, const float *styl
   PPlan *pl;
   FAV_TRY(build_pplan(p, H, W, &pl));
   p->last_plan = pl;
+  p->last_backward = false;
   FAV_TRY(check_cuda(cudaMemsetAsync(pl->overflow, 0, sizeof(int), st), "cudaMemsetAsync(overflow)"));
   // PerceptualCriterion.lua:85-93 then :117-155: capture the content targets, then the evaluated image in loss mode
   if (!p->content_tap.empty()) FAV_TRY(run_pass(p, *pl, content, 0, st));
@@ -1400,11 +1421,17 @@ int fav_percep_forward_backward(fav_percep_t *p, const float *content_pre, const
               "(k-1)/2 only", m, pc->k, pc->stride, pc->pad);
     return FAV_ERR_UNSUPPORTED;
   }
+  if (const int m = bwd_crowded_stage(p)) {
+    set_error("loss network module %d: too many loss layers between this convolution and the next (the backward pass takes %d, "
+              "or %d after the deepest convolution)", m, kMaxStageTerms - 1, kMaxStageTerms);
+    return FAV_ERR_UNSUPPORTED;
+  }
   FAV_TRY(prepare_backward(p));
   cudaStream_t st = (cudaStream_t)stream;
   PPlan *pl;
   FAV_TRY(build_pplan(p, H, W, &pl, true));
   p->last_plan = pl;
+  p->last_backward = true;
   FAV_TRY(check_cuda(cudaMemsetAsync(pl->overflow, 0, sizeof(int), st), "cudaMemsetAsync(overflow)"));
   // PerceptualCriterion.lua:117-134 (setContentTarget, then the input in loss mode), then :158-161
   if (!p->content_tap.empty()) FAV_TRY(run_pass(p, *pl, content_pre, 0, st, true));
@@ -1467,6 +1494,24 @@ int fav_percep_layer_output(fav_percep_t *p, int pass, int index, float *out, in
       return post_launch("percep_unpack_tap");
     }
   set_error("fav_percep_layer_output: layer %d is not a loss layer", index);
+  return FAV_ERR_INVALID;
+}
+
+int fav_percep_conv_output(fav_percep_t *p, int module_index, float *out, int *C, int *H, int *W, void *stream) {
+  FAV_REQUIRE(p && p->last_plan && p->last_backward, "fav_percep_conv_output: the last call was not fav_percep_forward_backward");
+  const PPlan *pl = p->last_plan;
+  for (size_t s = 0; s < p->convs.size(); ++s)
+    if (p->convs[s].module == module_index) {
+      const RawTensor &r = pl->raw[s];
+      if (C) *C = r.C;
+      if (H) *H = r.H;
+      if (W) *W = r.W;
+      if (!out) return FAV_OK;
+      percep_unpack_raw_kernel<<<dim3((unsigned)ceil_div64((int64_t)r.H * r.W, 256), r.C), 256, 0, (cudaStream_t)stream>>>(
+          r.p, r.Cq, r.Wp, r.C, r.H, r.W, out);
+      return post_launch("percep_unpack_raw");
+    }
+  set_error("fav_percep_conv_output: module %d is not a convolution of the trimmed loss network", module_index);
   return FAV_ERR_INVALID;
 }
 

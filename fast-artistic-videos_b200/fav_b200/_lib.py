@@ -95,6 +95,7 @@ SIGNATURES = {
     "fav_percep_evaluate": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), _fp]),
     "fav_percep_layer_output": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                           C.POINTER(C.c_int), _fp]),
+    "fav_percep_conv_output": (C.c_int, [C.c_void_p, C.c_int, _fp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), _fp]),
     "fav_percep_style_stat": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), _fp]),
     "fav_percep_forward_backward": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, _fp, C.POINTER(C.c_double),
                                               C.POINTER(C.c_double), C.POINTER(C.c_double), _fp]),

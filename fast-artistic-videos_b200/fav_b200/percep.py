@@ -160,6 +160,15 @@ class PerceptualCriterion:
         _lib.check(_lib.lib.fav_percep_layer_output(self._h, pass_, index, _lib.dptr(out), None, None, None, _lib.stream_ptr()))
         return out
 
+    def conv_output(self, module_index: int) -> torch.Tensor:
+        """fp32 output of convolution module `module_index` (bias included, before ReLU / pooling) from the last forward()
+        or backward() call: the values its ReLU masks and pooling arg-maxes were taken from.  [C,H,W] of the last image."""
+        c, h, w = C.c_int(), C.c_int(), C.c_int()
+        _lib.check(_lib.lib.fav_percep_conv_output(self._h, module_index, None, C.byref(c), C.byref(h), C.byref(w), None))
+        out = torch.empty((c.value, h.value, w.value), device="cuda", dtype=torch.float32)
+        _lib.check(_lib.lib.fav_percep_conv_output(self._h, module_index, _lib.dptr(out), None, None, None, _lib.stream_ptr()))
+        return out
+
     def forward(self, input: torch.Tensor, target) -> float:
         """percep_crit:forward(input, {content_target=...}) (PerceptualCriterion.lua:117-155, train_video.lua:343-344).
 

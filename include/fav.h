@@ -271,14 +271,26 @@ FAV_API int fav_percep_layer_output(fav_percep_t *p, int pass, int index, float 
                                     void *stream);
 /* tests: the aggregate (StyleLoss.lua:40-43) of style layer k (0-based position in the style layer list) as DEVICE
  * doubles: Gram matrix C*C (GramMatrix.lua:31-53) or C means; which 0 = style target, 1 = last evaluated image. */
+/* tests: the fp32 output (bias included, before any ReLU or pooling) of convolution module `module_index` from the last
+ * fav_percep_forward_backward, fp32 NCHW [C,H,W] (out may be NULL for the sizes): the values whose ReLU masks (> 0) and
+ * max-pooling arg-maxes the backward pass used.  FAV_ERR_INVALID if the last call was an evaluation or a style target (those
+ * share one buffer between convolutions) or the module is not a convolution. */
+FAV_API int fav_percep_conv_output(fav_percep_t *p, int module_index, float *out, int *C, int *H, int *W, void *stream);
 FAV_API int fav_percep_style_stat(fav_percep_t *p, int which, int k, double *out, int *n, void *stream);
 /* percep_crit:forward(input, {content_target=...}) then percep_crit:backward(input, target)   train_video.lua:343-345,
  * PerceptualCriterion.lua:117-161, ContentLoss.lua:50-59, StyleLoss.lua:57-67, GramMatrix.lua:54-78.
  * content_pre, input_pre [3,H,W] device fp32 in NET space (BGR, 255 x - mean; content_pre may be NULL without content layers);
  * writes grad_input [3,H,W] (d total / d input_pre), the two totals and, if layer_losses is not NULL, strength * MSE of every
- * loss layer (content layers, then style layers) through HOST doubles (synchronises `stream`).  Every convolution up to the
- * deepest loss layer must be stride 1 with pad (k-1)/2 (FAV_ERR_UNSUPPORTED naming the module otherwise, before any device
- * work).  The first call at a size keeps every convolution's fp32 output (about 1.1 GB at 1280x720 to relu4_3). */
+ * loss layer (content layers, then style layers) through HOST doubles (synchronises `stream`).  FAV_ERR_UNSUPPORTED names the
+ * module, before any kernel launch, unless every convolution up to the deepest loss layer
+ *  - is stride 1 with pad (k-1)/2, and
+ *  - has an input gradient (a nOutputPlane -> nInputPlane convolution) the tensor-core planner runs: nOutputPlane <= 8, or
+ *    nOutputPlane rounded up to 8 is an even number of 8-channel blocks (16, 32, 48, ...) that splits into at most 16 K groups
+ *    (blocks of 4 when the count is a multiple of 4, else of 2; a 5x5 or 7x7 filter over groups of 4 blocks, and a 7x7 over
+ *    groups of 2, takes a group per filter row).  Between convolutions only the deepest convolution's nOutputPlane is free, so e.g. 17, 33, 100, 130 or 200 there is
+ *    refused;
+ * and no convolution is followed by more than 7 loss layers before the next one (8 after the deepest).  The first call at a
+ * size keeps every convolution's fp32 output (about 1.1 GB at 1280x720 to relu4_3). */
 FAV_API int fav_percep_forward_backward(fav_percep_t *p, const float *content_pre, const float *input_pre, int H, int W,
                                         float *grad_input, double *content_loss, double *style_loss, double *layer_losses,
                                         void *stream);

@@ -23,6 +23,9 @@ def P(k, s, pad=0, ceil=False):
     return dict(type="pool", kW=k, kH=k, dW=s, dH=s, padW=pad, padH=pad, ceil_mode=ceil)
 
 
+P3x2 = dict(type="pool", kW=3, kH=2, dW=2, dH=1, padW=1, padH=0, ceil_mode=True)  # non-square window, stride and padding
+
+
 # (cin, cout, k, pad, stride, H, W, modules after the tested conv, aggregation, modules between the first conv and it)
 CASES = {
     # every wgmma width, Cout below the instance width
@@ -79,6 +82,17 @@ CASES = {
     "gram-c200-p129": (64, 200, 3, 1, 1, 3, 43, [R], "gram", None),
     "gram-c200-p127": (64, 200, 3, 1, 1, 1, 127, [R], "gram", None),
     "mean-c200-p128": (64, 200, 3, 1, 1, 2, 64, [R], "mean", None),
+    # poolings: non-square (3 wide, 2 tall, strides 2 / 1, padded in x only) at odd extents, and k2 s2 pad 1 ceil at extents
+    # 5 and 129, where the last ceil window would start in the padding and is dropped (pool_out)
+    "pool-k3x2-s2x1-ceil-odd": (16, 32, 3, 1, 1, 7, 131, [R, P3x2], "gram", None),
+    "pool-k2s2p1-ceil-drop": (16, 48, 3, 1, 1, 5, 129, [R, P(2, 2, 1, True)], "gram", None),
+    # input channels 32 / 96 / 112 / 192 / 208: the input gradient's wgmma N (32, 96, 112, and 128 + a partial 64 / 80 block)
+    "cin32-n16": (32, 16, 3, 1, 1, 4, 128, [R], "gram", None),
+    "cin48-k5-pool2s1": (48, 32, 5, 2, 1, 5, 131, [R, P(2, 1)], "gram", None),
+    "cin96-k5": (96, 64, 5, 2, 1, 3, 130, [R], "gram", None),
+    "cin112-pool3s1p1": (112, 32, 3, 1, 1, 4, 100, [R, P(3, 1, 1)], "gram", None),
+    "cin192": (192, 64, 3, 1, 1, 4, 130, [R], "gram", None),
+    "cin208-pool2": (208, 32, 3, 1, 1, 3, 129, [R, P(2, 2)], "mean", None),
 }
 
 
@@ -92,6 +106,55 @@ def test_case_table_covers_every_wgmma_width():
     widths = {n for case in CASES.values() for n in npads(case[1])}
     assert widths == set(range(16, 129, 16)), sorted(widths)
     assert npads(130) == [128, 16] and npads(300) == [128, 128, 48]
+
+
+def dgrad_plannable(cin, k):
+    """Whether the tensor-core planner runs a stride-1 k x k convolution over `cin` input channels (conv_plan.hpp:
+    build_phase_tables): 8 channels (tap pairing), or an even number of 8-channel blocks in K groups of 4 blocks (2 when the
+    count is not a multiple of 4), times the filter-row groups that keep one patch stage within 56 KB, at most 16 groups."""
+    blocks = -(-cin // 8)
+    if blocks == 1:
+        return True
+    if blocks % 2:
+        return False
+    cbg = 4 if blocks % 4 == 0 else 2
+    nrg = next(rg for rg in range(1, k + 1) if k % rg == 0 and (k // rg) * cbg * (128 + k - 1) * 32 <= 56 * 1024)
+    return nrg * (blocks // cbg) <= 16
+
+
+def backward_refusal(mods):
+    """(module index, reason) of the convolution fav_percep_forward_backward refuses, or None: first any stride != 1 or
+    pad != (k - 1) / 2, then the first input gradient (a cout -> cin convolution, so Cin = the forward's Cout) without a plan"""
+    convs = [(i, m) for i, m in enumerate(mods, 1) if m["type"] == "conv"]
+    for i, m in convs:
+        if m["stride"] != 1 or m["pad"] != (m["k"] - 1) // 2:
+            return i, "stride/pad"
+    for i, m in convs:
+        if not dgrad_plannable(m["cout"], m["k"]):
+            return i, "input gradient"
+    return None
+
+
+def dgrad_widths(name):
+    """wgmma N of every input-gradient convolution of a row's chain: N blocks of the forward Cin"""
+    mods = chain(name)[0]
+    return {n for m in mods if m["type"] == "conv" for n in npads(m["cin"])}
+
+
+def test_backward_rows_cover_every_input_gradient_width():
+    """The rows whose backward runs must reach every wgmma width of the input-gradient convolutions; trimming the table
+    must not drop one."""
+    runs = [name for name in CASES if backward_refusal(chain(name)[0]) is None]
+    widths = set().union(*(dgrad_widths(name) for name in runs))
+    assert widths == set(range(16, 129, 16)), sorted(widths)
+
+
+def test_backward_refusal_rules():
+    assert [c for c in (1, 3, 8, 16, 17, 24, 32, 33, 48, 64, 90, 100, 128, 130, 200, 300, 512) if not dgrad_plannable(c, 3)] == \
+        [17, 24, 33, 100, 130, 200, 300]
+    assert dgrad_plannable(64, 7) and not dgrad_plannable(48, 7) and dgrad_plannable(96, 5) and not dgrad_plannable(128, 5)
+    refused = [name for name in CASES if backward_refusal(chain(name)[0])]
+    assert len(CASES) - len(refused) == 29 and len(refused) == 26, (len(CASES), len(refused))
 
 
 def conv(rng, cin, cout, k, pad, stride):

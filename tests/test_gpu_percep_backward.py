@@ -1,23 +1,27 @@
 """The loss side of training on the GPU: PerceptualCriterion's forward + backward through the loss network
 (fav_percep_forward_backward, csrc/percep.cu), the pixel-loss gradient and the TotalVariation gradient, each against fp64
-torch.autograd over the same modules (seeded weights in VGG-16's real shapes)."""
+torch.autograd over the same modules: VGG-16's real shapes with seeded weights, and every geometry of the loss-network sweep
+(test_gpu_conv_geometry.CASES).  The loss network's gradient is checked at every pixel against an fp64 chain that takes the
+GPU's ReLU and pooling decisions (oracle/percep_grad_oracle.py)."""
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from fav_b200 import _lib, percep, synth
+from oracle import percep_grad_oracle as pgo
 from oracle import percep_oracle
+from test_gpu_conv_geometry import CASES as GEOMETRY, backward_refusal, chain, conv
+from test_gpu_percep import FEATURE_BAR, cuda
 
 pytestmark = pytest.mark.gpu
 
-# x max |ref|.  Where a pre-activation's fp64 value lies within the forward's rounding of 0 (or a pooling window's two largest
-# values do), the ReLU's (pooling's) gradient is discontinuous and either side is right; one such decision deep in the network
-# moves the gradient of its whole receptive field, a large share of a 64x96 input.  Measured on an H100: the 99th percentile
-# and the relative L2 error stay below 1.2e-2 in every case, the max error below 9e-2; a case without such a unit (the 3x3/2
-# pooling one) is 3e-5 off everywhere, and a loss on conv1_1's raw output (no ReLU or pooling on the path) 5e-6.
-GRAD_BAR = 2e-2
-EXACT_BAR = 1e-3  # max |got - ref| / max |ref| where no ReLU or pooling decision lies on the path
+# The reference gradient (oracle/percep_grad_oracle.py) takes the ReLU masks and pooling arg-maxes the backward pass read from
+# its fp32 conv outputs (fav_percep_conv_output), so it is a linear map of continuous values and is compared at every pixel:
+# max |got - ref| <= PIXEL_BAR x max |ref|, over the whole gradient and over its outer two rows and columns on their own.
+# Every unit where a GPU decision differs from the fp64 forward's own must lie within the forward's feature bar of the
+# discontinuity: |z| (or the window's fp64 gap to its maximum) <= FEATURE_BAR x max |z| of its conv output.
+PIXEL_BAR = pgo.PIXEL_BAR
+EXACT_BAR = 1e-3  # max |got - ref| / max |ref| against plain fp64 autograd, where no ReLU or pooling decision lies on the path
 # relative, totals and per-layer losses.  The style loss at relu4_3 is the MSE of (G - T) with G 1.3e-4 off fp64
 # (test_gpu_percep.py): 2.3e-4 measured on an H100 at 64x96
 LOSS_BAR = 5e-4
@@ -39,59 +43,33 @@ def images(H, W, seed):
     return content, stylized, style
 
 
-def features(mods, x, indices):
-    """percep_oracle.features from a net-space [1,3,H,W] tensor (differentiable)"""
-    want, out = set(indices), {}
-    for i, m in enumerate(mods[:max(want)], 1):
-        if m["type"] == "conv":
-            w = torch.as_tensor(np.asarray(m["weight"], np.float64), device=x.device)
-            b = torch.as_tensor(np.asarray(m["bias"], np.float64), device=x.device)
-            x = F.conv2d(x, w, b, stride=m["stride"], padding=m["pad"])
-        elif m["type"] == "relu":
-            x = torch.relu(x)
-        else:
-            x = F.max_pool2d(x, (m["kH"], m["kW"]), (m["dH"], m["dW"]), (m["padH"], m["padW"]), ceil_mode=bool(m["ceil_mode"]))
-        if i in want:
-            out[i] = x[0]
-    return out
-
-
-def aggregate(f, agg_type):
-    C, H, W = f.shape
-    x = f.reshape(C, H * W)
-    return x @ x.t() / (C * H * W) if agg_type == "gram" else x.mean(1)
-
-
-def oracle(mods, x, xc, cl, cw, sl, sw, targets, agg_type):
-    """fp64 autograd of PerceptualCriterion's output w.r.t. the net-space input: (grad [3,H,W], per-layer losses)"""
-    dev = "cuda"
-    X = x.to(dev, torch.float64)[None].requires_grad_()
-    fc = features(mods, xc.to(dev, torch.float64)[None], cl) if cl else {}
-    fs = features(mods, X, cl + sl)
-    per = [w * ((fs[i] - fc[i].detach()) ** 2).mean() for i, w in zip(cl, cw)]
-    per += [w * ((aggregate(fs[i], agg_type) - t.to(dev)) ** 2).mean() for i, w, t in zip(sl, sw, targets)]
-    (g,) = torch.autograd.grad(sum(per), X)
-    return g[0].cpu(), [float(v.detach()) for v in per]
-
-
 def rel_err(got, ref):
     got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
     assert got.shape == ref.shape, (got.shape, ref.shape)
     return float(np.abs(got - ref).max()) / float(np.abs(ref).max())
 
 
-def grad_err(got, ref):
-    """(99th percentile of |got - ref| / max |ref|, relative L2 error, max |got - ref| / max |ref|)"""
-    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
-    assert got.shape == ref.shape, (got.shape, ref.shape)
-    d, m = np.abs(got - ref), float(np.abs(ref).max())
-    return float(np.quantile(d, 0.99)) / m, float(np.linalg.norm(got - ref) / np.linalg.norm(ref)), float(d.max()) / m
-
-
-def check_grad(got, ref, what):
-    q, l2, mx = grad_err(got, ref)
-    print(f"  {what}: grad 99% {q:.1e}, L2 {l2:.1e}, max {mx:.1e} of max|ref| {float(np.abs(np.asarray(ref)).max()):.3e}")
-    assert q <= GRAD_BAR and l2 <= GRAD_BAR, (what, q, l2, mx)
+def check_backward(crit, mods, grad, x, xc, cl, cw, sl, sw, targets, agg_type, what, scale=1.0):
+    """The checks of one fav_percep_forward_backward result `grad` (x scale = the reference's factor) against the fixed-decision
+    fp64 reference; the conv outputs are those of the last call.  Returns (reference gradient, per-layer losses)."""
+    last = max(list(cl) + list(sl))
+    convs = [i for i, m in enumerate(mods[:last], 1) if m["type"] == "conv"]
+    raws = {i: crit.conv_output(i) for i in convs}
+    with torch.no_grad():
+        f64 = pgo.plain_features(mods, x.to("cuda", torch.float64), convs)
+    feat = max(rel_err(raws[i].cpu(), f64[i].cpu()) for i in convs)
+    del f64
+    ref, per, dec = pgo.grad(mods, x, xc, cl, cw, sl, sw, targets, agg_type, raws=raws, device="cuda")
+    ref = ref * scale
+    e, eb = pgo.pixel_err(grad, ref)
+    l2 = float(np.linalg.norm(np.asarray(grad, np.float64) - ref.numpy()) / np.linalg.norm(ref.numpy()))
+    ndiff, worst = sum(d[2] for d in dec), max([d[3] for d in dec], default=0.0)
+    print(f"  {what}: grad max {e:.1e}, border {eb:.1e}, L2 {l2:.1e} of max|ref| {float(ref.abs().max()):.3e}; conv outputs "
+          f"{feat:.1e}; {ndiff} decisions differ from fp64 (worst {worst:.1e})")
+    assert feat <= FEATURE_BAR, (what, feat)
+    assert e <= PIXEL_BAR and eb <= PIXEL_BAR, (what, e, eb)
+    assert worst <= FEATURE_BAR, (what, [d for d in dec if d[2]])
+    return ref, per
 
 
 def setup(mods, cl, cw, sl, sw, agg_type, style):
@@ -148,12 +126,13 @@ def test_grad_and_losses_vs_fp64_autograd(case):
     crit, targets = setup(mods, cl, cw, sl, sw, agg_type, style)
     x, xc = net_space(stylized), net_space(content)
     grad, tc, ts, lay = run(crit, x, xc)
-    ref, per = oracle(mods, x, xc, cl, cw, sl, sw, targets, agg_type)
+    print(f"\n{name} {H}x{W}:")
+    ref, per = check_backward(crit, mods, grad, x, xc, cl, cw, sl, sw, targets, agg_type, name)
     lay_e = [abs(a - b) / abs(b) for a, b in zip(lay, per)]
-    print(f"\n{name} {H}x{W}: layers " + " ".join(f"{v:.1e}" for v in lay_e))
-    check_grad(grad, ref, name)
+    print("  layers " + " ".join(f"{v:.1e}" for v in lay_e))
     if max(cl + sl) == 1:
-        assert grad_err(grad, ref)[2] <= EXACT_BAR
+        plain, _, _ = pgo.grad(mods, x, xc, cl, cw, sl, sw, targets, agg_type, device="cuda", plain=True)
+        assert rel_err(grad, plain) <= EXACT_BAR
     assert max(lay_e) <= LOSS_BAR, (name, lay_e)
     rc, rs = sum(per[:len(cl)]), sum(per[len(cl):])
     assert (not cl or abs(tc - rc) <= LOSS_BAR * abs(rc)) and (not sl or abs(ts - rs) <= LOSS_BAR * abs(rs)), (tc, rc, ts, rs)
@@ -180,13 +159,13 @@ def test_tiny_gradient_keeps_the_bar():
     mods = percep.vgg16_modules(22)
     content, stylized, style = images(64, 96, 6)
     x, xc = net_space(stylized), net_space(content)
-    ref1, _ = oracle(mods, x, xc, [9, 16], [1.0, 1.0], [], [], [], "gram")
+    ref1, _, _ = pgo.grad(mods, x, xc, [9, 16], [1.0, 1.0], [], [], [], "gram", device="cuda", plain=True)
     w = 1e-11 / float(ref1.abs().max())
     crit, _ = setup(mods, [9, 16], [w, w], [], [], "gram", style)
     grad, tc, _, _ = run(crit, x, xc)
-    ref, per = oracle(mods, x, xc, [9, 16], [w, w], [], [], [], "gram")
+    print()
+    ref, per = check_backward(crit, mods, grad, x, xc, [9, 16], [w, w], [], [], [], "gram", "tiny")
     assert float(ref.abs().max()) < 1e-10
-    check_grad(grad, ref, "tiny")
     assert abs(tc - sum(per)) <= LOSS_BAR * sum(per)
     # identical input and target: a zero gradient everywhere, zeros and not NaN
     grad0, tc0, _, _ = run(crit, xc, xc)
@@ -217,10 +196,15 @@ def test_batch_through_the_python_api():
     total = crit.forward(x, target)
     grad = crit.backward(x, target)
     assert grad.shape == (2, 3, H, W)
-    refs = [oracle(mods, x[n].cpu(), xc[n].cpu(), CONTENT_LAYERS, [1.5], STYLE_LAYERS, sw, targets, "gram") for n in range(2)]
-    per = [(a + b) / 2 for a, b in zip(refs[0][1], refs[1][1])]
+    print()
+    refs = []
     for n in range(2):
-        check_grad(grad[n].cpu(), refs[n][0] / 2, f"image {n}")
+        # the same image alone: bitwise the batch's gradient x N, and its conv outputs are the ones the batch decided from
+        gn, _, _, _ = run(crit, x[n].cpu(), xc[n].cpu())
+        assert torch.equal(gn * 0.5, grad[n].cpu())
+        refs.append(check_backward(crit, mods, grad[n].cpu(), x[n].cpu(), xc[n].cpu(), CONTENT_LAYERS, [1.5], STYLE_LAYERS, sw,
+                                   targets, "gram", f"image {n}", scale=0.5))
+    per = [(a + b) / 2 for a, b in zip(refs[0][1], refs[1][1])]
     assert abs(total - sum(per)) <= LOSS_BAR * sum(per)
     assert len(crit.content_losses) == 1 and len(crit.style_losses) == 4
     for got, ref in zip(crit.content_losses + crit.style_losses, per):
@@ -269,8 +253,80 @@ def test_grad_at_1280x720_vs_fp64_autograd():
     crit, targets = setup(mods, CONTENT_LAYERS, [1.5], STYLE_LAYERS, sw, "gram", style)
     x, xc = net_space(stylized), net_space(content)
     grad, tc, ts, lay = run(crit, x, xc)
-    ref, per = oracle(mods, x, xc, CONTENT_LAYERS, [1.5], STYLE_LAYERS, sw, targets, "gram")
+    print()
+    ref, per = check_backward(crit, mods, grad, x, xc, CONTENT_LAYERS, [1.5], STYLE_LAYERS, sw, targets, "gram", "1280x720")
     lay_e = [abs(a - b) / abs(b) for a, b in zip(lay, per)]
-    print("\n1280x720: layers " + " ".join(f"{v:.1e}" for v in lay_e))
-    check_grad(grad, ref, "1280x720")
+    print("  layers " + " ".join(f"{v:.1e}" for v in lay_e))
     assert max(lay_e) <= LOSS_BAR, lay_e
+
+
+def geometry_layers(mods, tested):
+    """the loss layers of test_gpu_conv_geometry: the tested conv's raw output and every module after it, content on the
+    first and the last"""
+    layers = list(range(tested, len(mods) + 1))
+    return [tested, layers[-1]], [1.0, 0.5], layers, [1.0 + 0.5 * i for i in range(len(layers))]
+
+
+def check_refused(crit, x, xc, content, stylized, module):
+    n0 = _lib.lib.fav_launch_count()
+    with pytest.raises(_lib.FavError) as e:
+        run(crit, x, xc)
+    assert e.value.status == _lib.FAV_ERR_UNSUPPORTED and f"module {module}:" in str(e.value), str(e.value)
+    assert _lib.lib.fav_launch_count() == n0
+    with pytest.raises(_lib.FavError) as e2:
+        crit.conv_output(1)  # no backward plan ran since the style target
+    assert e2.value.status == _lib.FAV_ERR_INVALID
+    cl, sl = crit.evaluate(cuda(content), cuda(stylized))
+    assert cl > 0 and sl > 0
+
+
+@pytest.mark.parametrize("name", list(GEOMETRY))
+def test_backward_over_the_geometry_table(name):
+    """Every loss-network geometry of the forward sweep either backpropagates under the per-pixel checks or is refused by
+    the rules (test_gpu_conv_geometry.backward_refusal) before any kernel runs, leaving evaluate working."""
+    mods, tested, H, W, agg = chain(name)
+    cl, cw, sl, sw = geometry_layers(mods, tested)
+    content, stylized, style = images(H, W, 7)
+    crit, targets = setup(mods, cl, cw, sl, sw, agg, style)
+    x, xc = net_space(stylized), net_space(content)
+    refusal = backward_refusal(mods)
+    print(f"\n{name} {H}x{W}: " + (f"refused at module {refusal[0]} ({refusal[1]})" if refusal else ""))
+    if refusal:
+        check_refused(crit, x, xc, content, stylized, refusal[0])
+        return
+    grad, tc, ts, lay = run(crit, x, xc)
+    _, per = check_backward(crit, mods, grad, x, xc, cl, cw, sl, sw, targets, agg, name)
+    lay_e = [abs(a - b) / abs(b) for a, b in zip(lay, per)]
+    assert max(lay_e) <= LOSS_BAR, lay_e
+    # the evaluate plans share one raw buffer: the hook answers for backward plans only
+    crit.evaluate(cuda(content), cuda(stylized))
+    with pytest.raises(_lib.FavError) as e:
+        crit.conv_output(tested)
+    assert e.value.status == _lib.FAV_ERR_INVALID
+    crit.close()
+
+
+def stage_terms_modules(n_relu, relu_after_pool):
+    rng = np.random.default_rng(40 + n_relu)
+    R = dict(type="relu")
+    mods = [conv(rng, 3, 16, 3, 1, 1)] + [dict(R) for _ in range(n_relu)] + [dict(type="pool", kW=2, kH=2, dW=2, dH=2, padW=0,
+                                                                                   padH=0, ceil_mode=False)]
+    mods += [dict(R)] * relu_after_pool + [conv(rng, 16, 32, 3, 1, 1), dict(R)]
+    return mods
+
+
+def test_seven_loss_layers_on_one_stage_and_an_eighth_refused():
+    """conv1's stage carries the raw conv, five ReLUs and the pooling as loss layers (content and style mixed) next to the
+    term of the next stage: the eight terms percep_bwd_stage_kernel takes.  One more loss layer there is refused."""
+    content, stylized, style = images(20, 36, 12)
+    x, xc = net_space(stylized), net_space(content)
+    mods = stage_terms_modules(5, 0)
+    cl, cw, sl, sw = [1, 4, 7, 9], [1.0, 0.5, 2.0, 0.3], [2, 3, 5, 6, 7, 9], [1.0, 1.5, 0.5, 2.0, 1.0, 0.7]
+    crit, targets = setup(mods, cl, cw, sl, sw, "gram", style)
+    grad, tc, ts, lay = run(crit, x, xc)
+    print()
+    _, per = check_backward(crit, mods, grad, x, xc, cl, cw, sl, sw, targets, "gram", "seven layers on stage 1")
+    assert max(abs(a - b) / abs(b) for a, b in zip(lay, per)) <= LOSS_BAR
+    mods = stage_terms_modules(5, 1)  # conv, five ReLUs, pooling, ReLU: eight loss layers before the next conv
+    crit, _ = setup(mods, [1, 4, 8, 10], cw, sl, sw, "gram", style)
+    check_refused(crit, x, xc, content, stylized, 1)
