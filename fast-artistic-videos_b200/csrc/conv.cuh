@@ -14,6 +14,18 @@ constexpr int kTileM = 128;  // output pixels per tile (two 64-row wgmma halves)
 constexpr int kTraceWords = 64;   // u64 words per CTA in the optional timeline buffer
 constexpr int kTraceUnits = 6;    // units (tiles) per CTA recorded
 
+// The fp16 pair x = hi + lo carries ~22 significant bits only while lo is an fp16 normal, i.e. for |x| >= 2^-3 (lo's normals
+// start at 2^-14).  A tensor packed multiplied by 2^pow2_scale_exp has its max |x| in [2^14, 2^15): clear of that floor and of
+// the fp16 maximum 65504.  maxbits: the float bits of max |x|; 0 (an all-zero tensor) gives 0.  |e| <= 126 keeps 2^e and 2^-e
+// normal.  The factor is exact, so it changes no rounding; whoever reads the fp32 result multiplies it by 2^-e.
+__host__ __device__ inline int pow2_scale_exp(unsigned maxbits) {
+  if (maxbits == 0) return 0;
+  int e = (int)((maxbits >> 23) & 0xff);  // floor(log2 max) + 127; subnormals as 2^-126
+  e = (e < 1 ? 1 : e) - 127;
+  e = 14 - e;
+  return e < -126 ? -126 : (e > 126 ? 126 : e);
+}
+
 // One K=16 step of the implicit GEMM: two K8 "units" (a unit = 8 input channels of one filter tap).
 // a_off16: offset (16-byte units) of the first unit's pixel 0 inside the shared-memory patch stage;
 // lbo16:   distance between the two units (= patch slab pitch when they are adjacent channel blocks,
@@ -109,6 +121,9 @@ struct ConvJob {
   // (16-byte units), raw (floats), out3 (floats), stats (doubles), nl_raw (float4 units), nl_sums (doubles)
   int nimg;
   int64_t a_img16, raw_img, out3_img, stats_img, nl_raw_img4, nl_sums_img;
+  // the weights are packed multiplied by 2^w_exp (ConvDef::w_exp): every epilogue takes acc * w_unscale = acc * 2^-w_exp before
+  // the bias.  The operand epilogue has it folded into epi_scale instead.
+  float w_unscale;
 };
 
 // Tile T of a batched job, T = b * ntiles + t for image b and tile t of that image's output (0 <= T < nimg * ntiles): every role

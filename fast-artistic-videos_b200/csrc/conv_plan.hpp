@@ -3,6 +3,7 @@
 // code is exercised on the CPU by tests/emu (an emulation of the kernel's addressing) and on the GPU by net.cu.
 #pragma once
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -68,6 +69,9 @@ struct ConvDef {
   float *d_stack_bias = nullptr;
   float *d_bias = nullptr;
   float *d_scale = nullptr;  // batch-normalized nets: the per-channel BN scale the operand epilogue applies (Npad floats)
+  // the tensor cores multiply with the weights times 2^w_exp (set_weight_prescale): one exponent for the whole convolution,
+  // shared by its N blocks, sub-pixel phases and stacked jobs; fill_conv_job hands each job the factor 2^-w_exp
+  int w_exp = 0;
   int pw = -1, pb = -1;  // param indices
 };
 
@@ -254,6 +258,34 @@ static inline float h2f_bits(uint16_t b) {
   return __half2float(h);
 }
 
+// part 0 (hi) or 1 (lo) of the fp16 pair hi + lo of weight v packed at exponent e: v 2^e = hi + lo to ~2^-22 relative while
+// |v 2^e| >= 2^-3 (pow2_scale_exp, conv.cuh)
+static inline uint16_t weight_half(float v, int e, int part) {
+  const float s = ldexpf(v, e);
+  const uint16_t hb = f2h_bits(s);
+  return part == 0 ? hb : f2h_bits(s - h2f_bits(hb));
+}
+// ConvDef::w_exp for weights w: 0 while max |w| lies in [kWeightUnscaledMin, 2^15), else the exponent that puts max |w| 2^w_exp in
+// [2^14, 2^15) (0 when every weight is zero).  Unscaled, the split of any weight is off by at most 2^-25 (lo's subnormal step is
+// 2^-24), which above 2^-6 is at most 2^-19 of max |w|: no more than the fp32 accumulation's own error over K ~ 10^3 products, and
+// default-init nets (max |w| 2^-6 ... 2^-4) measure the same against fp64 either way.  Such convs keep the unscaled packing bit
+// for bit, so every output of the nets that use them stays the same, the recurrent clip included: a frame's last-bit change
+// grows to O(1) differences within 50 frames.  Below 2^-6 the split's error grows as 1 / max |w| and the scale takes over.
+static constexpr float kWeightUnscaledMin = 1.f / 64;
+static inline int weight_prescale_exp(const std::vector<float> &w) {
+  float m = 0.f;
+  for (float v : w) m = std::max(m, std::fabs(v));
+  if (m >= kWeightUnscaledMin && m < 32768.f) return 0;
+  unsigned bits;
+  memcpy(&bits, &m, 4);
+  return pow2_scale_exp(bits);
+}
+// the exponent of the whole convolution c with weights w, for c and each of its N blocks: set before any of them is packed
+static inline void set_weight_prescale(ConvDef &c, const std::vector<float> &w) {
+  c.w_exp = weight_prescale_exp(w);
+  for (ConvDef &cb : c.nblock) cb.w_exp = c.w_exp;
+}
+
 static inline float weight_at(const ConvDef &c, const std::vector<float> &w, int co, int ci, int ky, int kx) {
   if (co >= c.cout || ci >= c.cin) return 0.f;
   if (c.transposed) return w[(((int64_t)ci * c.cout + co) * c.k + ky) * c.k + kx];
@@ -304,9 +336,8 @@ static inline std::vector<uint16_t> pack_phase_fold(const ConvDef &c, const Conv
               for (int co = 0; co < c.cout; ++co)
                 for (int i = 0; i < 8; ++i) {
                   float v = (ky >= 0 && ky < c.k && kx >= 0 && kx < c.k) ? weight_at(c, w, co, cb * 8 + i, ky, kx) : 0.f;
-                  uint16_t hb = f2h_bits(v);
                   size_t o = base + ((((size_t)part * spc + j) * 2 + u) * n + (size_t)bi * c.cout + co) * 8 + i;
-                  pk[o] = part == 0 ? hb : f2h_bits(v - h2f_bits(hb));
+                  pk[o] = weight_half(v, c.w_exp, part);
                 }
             }
           }
@@ -496,9 +527,8 @@ static inline std::vector<uint16_t> pack_phase_weights(const ConvDef &c, const C
                 } else {              // kind 1: unit.tap = kx, cblk = co
                   v = weight_at(c, w, cblk, i, ky, un.tap);
                 }
-                uint16_t hb = f2h_bits(v);
                 size_t o = ((((size_t)st * 2 + part) * 2 + u) * NR + (size_t)(KH - 1 - ky) * Nblk + cblk) * 8 + i;
-                pk[o] = part == 0 ? hb : f2h_bits(v - h2f_bits(hb));
+                pk[o] = weight_half(v, c.w_exp, part);
               }
         }
     return pk;
@@ -528,8 +558,7 @@ static inline std::vector<uint16_t> pack_phase_weights(const ConvDef &c, const C
                 } else {
                   v = weight_at(c, w, n, un.cb * 8 + i, ph.taps[un.tap].ky, ph.taps[un.tap].kx);
                 }
-                uint16_t hb = f2h_bits(v);
-                pk[base + (size_t)n * 8 + i] = part == 0 ? hb : f2h_bits(v - h2f_bits(hb));
+                pk[base + (size_t)n * 8 + i] = weight_half(v, c.w_exp, part);
               }
           }
   return pk;
@@ -603,6 +632,7 @@ static inline int fill_conv_job(const ConvDef &c, const ConvPhase &ph, const Ope
   j.nchunks = ph.nchunks; j.spc = ph.spc;
   for (size_t i = 0; i < ph.steps.size(); ++i) j.steps[i] = ph.steps[i];
   j.chunk16 = 2 * ph.spc * 2 * ph.Npad; j.Npad = ph.Npad; j.Cout = c.cout;
+  j.w_unscale = ldexpf(1.f, -c.w_exp);
   if (ph.rf_R) { j.nchunks = j.rf_steps; j.spc = 1; j.chunk16 = 2 * 2 * j.rf_kh * ph.Npad; }  // one resident chunk per K step
   if (ph.pf) {
     j.pf = 1; j.pf_cout = c.cout; j.mt = 1;

@@ -7,7 +7,8 @@
 //   K = taps x input channels, walked in K=16 steps (two 8-channel "units" per step).
 // Precision: the reference computes in fp32.  A single fp16/tf32 pass misses the 1e-3 parity bar
 // (measured 1.2e-3..2.7e-3, DESIGN.md §precision), so every operand is an fp16 pair x = hi + lo and each
-// K step issues three MMAs  hi*hi + lo*hi + hi*lo  (fp32 accumulation): ~2^-21 relative error.
+// K step issues three MMAs  hi*hi + lo*hi + hi*lo  (fp32 accumulation): ~2^-21 relative error while |x| >= 2^-3, which the
+// weights get from a power-of-two prescale undone in the epilogue (ConvJob::w_unscale, DESIGN.md §2).
 //
 // Data movement: the input patch of a tile (all filter rows x a group of channel blocks x 128+halo pixels)
 // is fetched ONCE per tile by 1-D bulk async copies (cp.async.bulk, completion on an mbarrier).  Because the
@@ -177,9 +178,11 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
       }
       if (job.dbg & 8) continue;
 
-      // ===== epilogue from registers: acc[4i + 2h + e] = (pixel r0 + 8h, column 8i + q2 + e) =====
+      // ===== epilogue from registers: acc[4i + 2h + e] = (pixel r0 + 8h, column 8i + q2 + e), in units of the weights times
+      // 2^w_exp: every store takes acc * 2^-w_exp (exact) before the bias =====
       const TileAt at = tile_at(job, tile, BATCH);  // y, x0; the image's offsets are img's
       const int x0 = at.x0, y = at.y, yo = y * job.oy_mul + job.oy_off;
+      const float ws = OPND ? 1.f : job.w_unscale;  // the operand epilogue's epi_scale includes it
       if (job.xfold_kw) {
         // partial sums Q[pixel][kx*Cout + co] -> shared memory, then out[x][co] = sum_kx Q[x + kx][kx*Cout + co]
         const int ncol = job.xfold_kw * job.Cout;
@@ -190,7 +193,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int col = 8 * i + q2 + e;
-              if (col < ncol) exch[(r0 + 8 * h) * kExchPitch + col] = acc[4 * i + 2 * h + e];
+              if (col < ncol) exch[(r0 + 8 * h) * kExchPitch + col] = acc[4 * i + 2 * h + e] * ws;
             }
         asm volatile("bar.sync 1, 256;" ::: "memory");
         const int px = threadIdx.x, x = x0 + px;
@@ -224,7 +227,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
             const int k = q2 + e;
             if (k < 3 && k < job.Cout && valid[h])
               job.out3[img.out3 + ((int64_t)(job.final_mode == 2 ? 2 - k : k) * job.Ho + yo) * job.Wo + xo[h]] =
-                  tc_final_value(acc[2 * h + e] + __ldg(job.bias + k), k, job.final_mode, job.tanh_c);
+                  tc_final_value(fmaf(acc[2 * h + e], ws, __ldg(job.bias + k)), k, job.final_mode, job.tanh_c);
           }
         continue;
       }
@@ -241,8 +244,8 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   #pragma unroll
           for (int h = 0; h < 2; ++h) {
             int64_t o = 0;
-            v[2 * h] = acc[4 * i + 2 * h] + b.x;
-            v[2 * h + 1] = acc[4 * i + 2 * h + 1] + b.y;
+            v[2 * h] = fmaf(acc[4 * i + 2 * h], ws, b.x);
+            v[2 * h + 1] = fmaf(acc[4 * i + 2 * h + 1], ws, b.y);
             if (stack_epi_addr(job, y, x0, threadIdx.x, i, h, o) && !(job.dbg & 1))
               *reinterpret_cast<float2 *>(raw + o) = make_float2(v[2 * h], v[2 * h + 1]);
             else
@@ -259,7 +262,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   #pragma unroll
         for (int i = 0; i < NJ; ++i) {
           const int c = 8 * i + q2;
-          // bias and scale are padded to Npad
+          // bias and scale are padded to Npad; the scale includes the weights' 2^-w_exp (pack_conv_weights, net.cu)
           const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c)), s = __ldg(reinterpret_cast<const float2 *>(job.epi_scale + c));
   #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -292,8 +295,8 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
         float v[4];
   #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          v[2 * h] = acc[4 * i + 2 * h] + b.x;
-          v[2 * h + 1] = acc[4 * i + 2 * h + 1] + b.y;
+          v[2 * h] = fmaf(acc[4 * i + 2 * h], ws, b.x);
+          v[2 * h + 1] = fmaf(acc[4 * i + 2 * h + 1], ws, b.y);
           // raw layout [Ho][Cq][Wp][4]: channels c, c + 1 of one pixel are 8 contiguous bytes
           if (valid[h] && c < job.Cout)
             *reinterpret_cast<float2 *>(raw + (((int64_t)yo * job.raw_Cq + (c >> 2)) * job.raw_Wp + xo[h]) * 4 + (c & 3)) =

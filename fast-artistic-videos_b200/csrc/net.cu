@@ -219,12 +219,14 @@ static int pack_tc_weights(fav_net *net, ConvDef &c, const std::vector<float> &w
 }
 
 // w: the weights the tensor cores multiply with, b the bias; w_simt: the CUDA-core comparator's weights; scale: empty, or the
-// per-channel BatchNorm scale the operand epilogue applies (fold_batch_norms)
+// per-channel BatchNorm scale the operand epilogue applies (fold_batch_norms).  The tensor cores get w times 2^c.w_exp
+// (set_weight_prescale); the operand epilogue takes the 2^-w_exp back with the scale, every other epilogue from ConvJob::w_unscale.
 static int pack_conv_weights(fav_net *net, ConvDef &c, const std::vector<float> &w, const std::vector<float> &b,
                              const std::vector<float> &w_simt, const std::vector<float> &scale) {
+  set_weight_prescale(c, w);
   std::vector<float> bias(c.Npad, 0.f), sc(c.Npad, 0.f);
   for (int i = 0; i < c.cout; ++i) bias[i] = b[i];
-  for (size_t i = 0; i < scale.size(); ++i) sc[i] = scale[i];
+  for (size_t i = 0; i < scale.size(); ++i) sc[i] = ldexpf(scale[i], -c.w_exp);
   FAV_TRY(dev_upload(net, bias, &c.d_bias));
   if (!scale.empty()) FAV_TRY(dev_upload(net, sc, &c.d_scale));
   for (size_t b = 0; b < c.nblock.size(); ++b) {  // N blocks: weight, bias and scale slices

@@ -352,12 +352,9 @@ __global__ void __launch_bounds__(256) percep_unpack_raw_kernel(const float *__r
 // packed multiplied by a per-tensor power of two that maps its max |g| into [2^14, 2^15).  The factor is exact, so it changes no
 // rounding; the kernel that reads the convolution's fp32 output divides it out.  The max lives in device memory.
 
-// 2^k for max |g| (float bits) in [2^(14-k), 2^(15-k)); 1 for an all-zero tensor.  |k| <= 126 keeps 2^k and 2^-k normal.
-__device__ __forceinline__ int grad_scale_exp(unsigned maxbits) {
-  if (maxbits == 0) return 0;
-  const int e = max((int)((maxbits >> 23) & 0xff), 1) - 127;  // floor(log2 max); subnormals as 2^-126
-  return min(max(14 - e, -126), 126);
-}
+// 2^k for max |g| (float bits) in [2^(14-k), 2^(15-k)); 1 for an all-zero tensor (pow2_scale_exp, conv.cuh).  The weights of
+// every convolution get the same treatment once, on the host (weight_prescale_exp, conv_plan.hpp).
+__device__ __forceinline__ int grad_scale_exp(unsigned maxbits) { return pow2_scale_exp(maxbits); }
 __device__ __forceinline__ float grad_scale(unsigned maxbits) { return ldexpf(1.f, grad_scale_exp(maxbits)); }
 __device__ __forceinline__ float grad_unscale(unsigned maxbits) { return ldexpf(1.f, -grad_scale_exp(maxbits)); }
 
@@ -1094,9 +1091,11 @@ static int prepare_backward(fav_percep *P) {
           for (int kx = 0; kx < k; ++kx)
             wt[(((size_t)ci * pc.cout + co) * k + ky) * k + kx] = pc.w[(((size_t)co * pc.cin + ci) * k + (k - 1 - ky)) * k + (k - 1 - kx)];
     std::vector<ConvDef> blocks;
+    const int w_exp = weight_prescale_exp(wt);  // one exponent for every N block (set_weight_prescale)
     for (int b = 0; b < conv_nblocks(pc.cin); ++b) {
       ConvDef c;
       init_nblock_conv_def(c, "percep_dgrad" + std::to_string(pc.module), pc.cout, pc.cin, k, 1, pc.pad, b);
+      c.w_exp = w_exp;
       if (build_phase_tables(c, c.phases[0]) != FAV_OK) {
         set_error("loss network module %d: the input gradient (convolution %d->%d k%d) is not a geometry the tensor-core planner runs",
                   pc.module, pc.cout, pc.cin, k);
@@ -1344,9 +1343,11 @@ int fav_percep_finalize(fav_percep_t *p) {
     return FAV_ERR_UNSUPPORTED;
   }
   p->num_sms = prop.multiProcessorCount;
-  for (PConv &pc : p->convs)
+  for (PConv &pc : p->convs) {
+    const int w_exp = weight_prescale_exp(pc.w);  // one exponent for every N block (set_weight_prescale)
     for (size_t b = 0; b < pc.blocks.size(); ++b) {
       ConvDef &c = pc.blocks[b];
+      c.w_exp = w_exp;
       const std::vector<float> w = conv_nblock_weights(pc.w, pc.cin, pc.cout, pc.k, (int)b);
       std::vector<uint16_t> pk = pack_phase_weights(c, c.phases[0], w);
       void *d = nullptr;
@@ -1360,6 +1361,7 @@ int fav_percep_finalize(fav_percep_t *p) {
       FAV_TRY(check_cuda(cudaMemcpy(db, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice), "cudaMemcpy(percep bias)"));
       pc.d_bias.push_back(db);
     }
+  }
   for (size_t k = 0; k < p->style_tap.size(); ++k) {
     const int C = p->convs[p->taps[p->style_tap[k]].stage].cout;
     double *t = nullptr, *s = nullptr;

@@ -77,6 +77,7 @@ extern "C" int emu_conv_check(int cin, int cout, int k, int stride, int pad, int
   std::vector<char> written((size_t)Ho * Wo, 0);
   int mma_count = 0;
   size_t smem_max = 0;
+  set_weight_prescale(c, w);
   std::vector<ConvPhase *> todo;
   if (c.has_fold) todo.push_back(&c.fold);
   else for (ConvPhase &p : c.phases) todo.push_back(&p);
@@ -230,6 +231,7 @@ extern "C" int emu_conv_check(int cin, int cout, int k, int stride, int pad, int
       // epilogue: K-split units add the second warp's accumulator
       if (j.ksplit)
         for (size_t i = 0; i < acc.size(); ++i) acc[i] += acc2[i];
+      for (double &v : acc) v *= j.w_unscale;  // the packed weights are w * 2^w_exp
       // epilogue placement
       if (j.rf_R) {
         const int nblk = j.rf_nblk;
@@ -365,5 +367,163 @@ extern "C" int emu_plan_detail(int cin, int cout, int k, int stride, int pad, in
   const int v[16] = {j.ngroups, j.nchunks, j.spc, j.nrows, j.CbG, j.nseg, j.a_stages, j.b_slots, j.b_resident, j.stage16 * 16,
                      j.chunk16 * 16, j.pslab16, j.tiles_x, j.ntiles, j.Npad, j.ksplit};
   for (int i = 0; i < 16; ++i) out16[i] = v[i];
+  return 0;
+}
+
+// ---- weight prescale (set_weight_prescale, weight_half): every packing path against the weights it packs -----------------
+// A packed job does not say which weight each of its fp16 pairs holds, so the job is packed twice: once from the weights and
+// once from their indices (index i + 1 as the weight value; max < 2^22, so hi + lo holds it exactly).  Position p then holds
+// weight idx[p] and must decode, as hi + lo times the job's 2^-w_exp, to within 2^-21 of it: relative to the weight itself, or to
+// the pair's floor 2^-4 in packed units (2^-4-e in weight units): lo's subnormal step 2^-24 bounds the error by 2^-25.
+struct PackedJob {
+  ConvDef c;            // the ConvDef the job is packed from (an N block, or the whole convolution)
+  const ConvPhase *ph;  // the phase (tables) it packs
+  std::vector<float> w, idx;
+  int path;             // 0: pack_phase_weights, 1: row-fold image, 2: pack_phase_fold
+  int e;                // the exponent the job runs with: ConvJob::w_unscale = 2^-e (row-fold: ConvDef::w_exp)
+};
+
+// distance (uint16 elements) from each hi element to its lo partner, and whether element p is a hi element
+static bool hi_element(const PackedJob &pj, size_t p, size_t *lo_off) {
+  const ConvPhase &ph = *pj.ph;
+  if (pj.path == 1) {  // [step][hi|lo][k-half][NR][8]
+    const size_t B = (size_t)2 * ph.rows.size() * ph.Npad * 8;
+    *lo_off = B;
+    return (p / B) % 2 == 0;
+  }
+  if (pj.path == 2) {  // [group][tap chunk: [hi|lo][spc][k-half][n][8]]
+    const int spc = ph.CbG / 2;
+    size_t grp = 0;
+    for (int t = 0; t < 4; ++t) grp += (size_t)2 * spc * 2 * kPfNblk[t] * pj.c.cout * 8;
+    size_t q = p % grp;
+    for (int t = 0; t < 4; ++t) {
+      const size_t B = (size_t)spc * 2 * kPfNblk[t] * pj.c.cout * 8;
+      if (q < 2 * B) { *lo_off = B; return q < B; }
+      q -= 2 * B;
+    }
+    return false;
+  }
+  const size_t B = (size_t)ph.spc * 2 * ph.Npad * 8;  // [group][chunk][hi|lo][step][k-half][Npad][8]
+  *lo_off = B;
+  return (p / B) % 2 == 0;
+}
+
+static std::vector<uint16_t> pack_job(const PackedJob &pj, const ConvDef &c, const std::vector<float> &w) {
+  return pj.path == 2 ? pack_phase_fold(c, *pj.ph, w) : pack_phase_weights(c, *pj.ph, w);
+}
+
+// the row-fold tables build_phase_tables gives a tap-paired (kind 1) or x-fold (kind 3) phase when kPlanRowFold is on: the K
+// steps of one patch row, all channel blocks in one stage
+static void rowfold_tables(const ConvDef &c, ConvPhase &ph) {
+  ph.steps.clear();
+  ph.units.assign(1, {});
+  if (ph.kind == 1) {
+    const int ndx = ph.dxmax - ph.dxmin + 1;
+    for (int p = 0; p * 2 < ndx; ++p) {
+      ph.steps.push_back(KStep{(uint16_t)(2 * p), 1});
+      for (int u = 0; u < 2; ++u) ph.units[0].push_back(Unit{2 * p + u < ndx ? 2 * p + u : -1, 0});
+    }
+  } else {
+    ph.CbG = c.Cb; ph.nchg = 1;
+    for (int j = 0; j < ph.CbG / 2; ++j) {
+      ph.steps.push_back(KStep{(uint16_t)(2 * j * ph.pslab16), (uint16_t)ph.pslab16});
+      for (int u = 0; u < 2; ++u) ph.units[0].push_back(Unit{0, 2 * j + u});
+    }
+  }
+  ph.rf_R = 4; ph.nrg = 1; ph.spc = (int)ph.steps.size(); ph.nchunks = 1;
+}
+
+// path 0: every job the stylization net / loss network packs for the convolution (N blocks x sub-pixel phases, stacked phases,
+// x-fold when !raw_out); 1: the row-fold image of its first phase (tap-paired or x-fold); 2: the phase-fold job (f3s2).
+// Weights U(-1, 1)^3 * wscale (0: all zero).  out: [0] worst error / bound, [1] max |w| 2^e, [2] jobs, [3] distinct exponents,
+// [4] weights no job packs.  *e_out: the exponent of the first job.
+extern "C" int emu_weight_scale_check(int cin, int cout, int k, int stride, int pad, int transposed, int adj, int raw_out, int path,
+                                      double wscale, unsigned seed, double *out, int *e_out) {
+  ConvDef c;
+  init_conv_def(c, "emu", cin, cout, k, stride, pad, transposed != 0, adj);
+  build_phases(c);
+  c.raw_out = raw_out != 0;
+  std::mt19937 rng(seed);
+  std::uniform_real_distribution<double> U(-1.0, 1.0);
+  std::vector<float> w((size_t)cin * cout * k * k), idx(w.size());
+  double maxw = 0;
+  for (size_t i = 0; i < w.size(); ++i) {
+    const double u = U(rng);
+    w[i] = (float)(u * u * u * wscale);
+    if (i == 0) w[i] = (float)(0.999 * wscale);  // one weight near the top of the binade
+    idx[i] = (float)(i + 1);
+    maxw = std::max(maxw, (double)std::fabs(w[i]));
+  }
+  if (idx.size() >= (1u << 22)) { set_error("too many weights to index exactly"); return 1; }
+  Operand op = operand_geometry(cin, 16, 16, &c);
+  std::vector<PackedJob> jobs;
+  std::vector<ConvPhase> extra;  // row-fold / phase-fold tables
+  extra.reserve(1);
+  if (path == 0) {
+    if (plan_conv_nblocks(c) != FAV_OK || plan_phase_stack(c) != FAV_OK) return 2;
+    set_weight_prescale(c, w);
+    if (!c.nblock.empty()) {
+      for (int b = 0; b < (int)c.nblock.size(); ++b)
+        for (const ConvPhase &ph : c.nblock[b].phases)
+          jobs.push_back(PackedJob{c.nblock[b], &ph, conv_nblock_weights(w, cin, cout, k, b, c.transposed),
+                                   conv_nblock_weights(idx, cin, cout, k, b, c.transposed), 0, 0});
+    } else {
+      for (const ConvPhase &ph : c.phases) jobs.push_back(PackedJob{c, &ph, w, idx, 0, 0});
+    }
+    for (const ConvPhase &ph : c.stack) jobs.push_back(PackedJob{c, &ph, w, idx, 0, 0});
+  } else if (path == 1) {
+    extra.push_back(c.phases[0]);
+    if (build_phase_tables(c, extra[0]) != FAV_OK) return 2;
+    if (extra[0].kind != 1 && extra[0].kind != 3) { set_error("row-fold needs a tap-paired or x-fold phase, got kind %d", extra[0].kind); return 3; }
+    rowfold_tables(c, extra[0]);
+    set_weight_prescale(c, w);
+    jobs.push_back(PackedJob{c, &extra[0], w, idx, 1, 0});
+  } else {
+    extra.push_back(ConvPhase());
+    if (build_phase_fold(c, extra[0]) != FAV_OK) { set_error("no phase-fold plan"); return 3; }
+    set_weight_prescale(c, w);
+    jobs.push_back(PackedJob{c, &extra[0], w, idx, 2, 0});
+  }
+  std::vector<int> seen(w.size(), 0), exps;
+  double worst = 0;
+  for (PackedJob &pj : jobs) {
+    if (pj.path == 1) {
+      pj.e = pj.c.w_exp;
+    } else {
+      ConvJob j;
+      if (fill_conv_job(pj.c, *pj.ph, op, j) != FAV_OK) return 4;
+      pj.e = -ilogbf(j.w_unscale);
+      if (j.w_unscale != ldexpf(1.f, -pj.e)) { set_error("w_unscale %g is not a power of two", j.w_unscale); return 5; }
+    }
+    if (std::find(exps.begin(), exps.end(), pj.e) == exps.end()) exps.push_back(pj.e);
+    const std::vector<uint16_t> pw = pack_job(pj, pj.c, pj.w);
+    ConvDef ci = pj.c;
+    ci.w_exp = weight_prescale_exp(pj.idx);
+    const std::vector<uint16_t> pi = pack_job(pj, ci, pj.idx);
+    if (pw.size() != pi.size()) { set_error("packed sizes differ"); return 6; }
+    for (size_t p = 0; p < pw.size(); ++p) {
+      size_t lo_off = 0;
+      if (!hi_element(pj, p, &lo_off)) continue;
+      if (p + lo_off >= pw.size()) { set_error("lo element out of range"); return 7; }
+      const double id = ldexp((double)h2f_bits(pi[p]) + h2f_bits(pi[p + lo_off]), -ci.w_exp);
+      const double got = ldexp((double)h2f_bits(pw[p]) + h2f_bits(pw[p + lo_off]), -pj.e);
+      if (id == 0) {  // a zero tap or padding
+        if (pw[p] != 0 || pw[p + lo_off] != 0) { set_error("padding element %zu holds %g", p, got); return 8; }
+        continue;
+      }
+      const long long i = std::llround(id) - 1;
+      if (i < 0 || i >= (long long)w.size() || (double)(i + 1) != id) { set_error("element %zu decodes to index %g", p, id); return 9; }
+      seen[i]++;
+      const double ref = w[i], err = std::fabs(got - ref);
+      const double bound = std::ldexp(std::max(std::fabs(ref), std::ldexp(1.0, -4 - pj.e)), -21);
+      const double r = bound > 0 ? err / bound : (err > 0 ? 1e300 : 0.0);
+      if (!(r <= worst)) worst = std::isnan(r) ? 1e300 : r;
+    }
+  }
+  int unseen = 0;
+  for (int s : seen) unseen += s == 0;
+  out[0] = worst; out[1] = std::ldexp(maxw, jobs[0].e); out[2] = (double)jobs.size(); out[3] = (double)exps.size();
+  out[4] = unseen;
+  *e_out = jobs[0].e;
   return 0;
 }

@@ -36,6 +36,7 @@ extern "C" int emu_nblock_check(int cin, int cout, int k, int pad, int H, int W,
   for (int b = 0; b < nb; ++b) {
     ConvDef c;
     init_nblock_conv_def(c, "emu", cin, cout, k, 1, pad, b);
+    c.w_exp = weight_prescale_exp(w);  // the whole convolution's exponent (set_weight_prescale)
     ConvPhase &ph = c.phases[0];
     if (build_phase_tables(c, ph) != FAV_OK) return 1;
     if (ph.kind != 0 && ph.kind != 1) { set_error("N-block job planned as kind %d", ph.kind); return 12; }
@@ -95,7 +96,7 @@ extern "C" int emu_nblock_check(int cin, int cout, int k, int pad, int H, int W,
         for (int n = 0; n < j.Cout; ++n) {
           const int64_t o = raw_off + (((int64_t)y * Cq + (n >> 2)) * Wp + xx) * 4 + (n & 3);
           if (o < 0 || o >= (int64_t)raw.size()) { set_error("raw OOB"); return 7; }
-          raw[o] = acc[(size_t)m * Npad + n];
+          raw[o] = acc[(size_t)m * Npad + n] * j.w_unscale;
           written[o]++;
         }
       }

@@ -65,6 +65,7 @@ extern "C" int emu_stack_check(int cin, int cout, int k, int H, int W, unsigned 
   std::vector<double> raw((size_t)Ho * Cq * Wp * 4, 0.0), ssum(cout, 0.0), ssq(cout, 0.0);
   std::vector<int> written(raw.size(), 0);
   const std::vector<float> sb = stack_bias(c, bias);
+  set_weight_prescale(c, w);
   for (const ConvPhase &ph : c.stack) {
     const std::vector<uint16_t> pk = pack_phase_weights(c, ph, w);
     ConvJob j;
@@ -128,7 +129,7 @@ extern "C" int emu_stack_check(int cin, int cout, int k, int H, int W, unsigned 
             if (o < 0 || o + 1 >= (int64_t)raw.size()) { set_error("epilogue address out of range"); return 8; }
             for (int e = 0; e < 2; ++e) {
               const int n = 8 * i + 2 * (t & 3) + e;
-              const double v = acc[(size_t)(r0 + 8 * h) * Npad + n] + sb[n];
+              const double v = acc[(size_t)(r0 + 8 * h) * Npad + n] * j.w_unscale + sb[n];
               raw[o + e] = v;
               written[o + e]++;
               col_sum[n] += v;

@@ -23,6 +23,7 @@ extern "C" int emu_style_nblock_check(int cin, int cout, int k, int stride, int 
   c.raw_out = true;
   if (plan_conv_nblocks(c) != FAV_OK) return 1;
   if ((int)c.nblock.size() != conv_nblocks(cout)) { set_error("%d N blocks planned", (int)c.nblock.size()); return 12; }
+  set_weight_prescale(c, w);
   Operand op = operand_geometry(cin, H, W, &c);
   std::vector<uint16_t> hi(op.elems16 * 8, 0), lo(op.elems16 * 8, 0);
   std::vector<float> xq((size_t)cin * H * W);
@@ -108,7 +109,7 @@ extern "C" int emu_style_nblock_check(int cin, int cout, int k, int stride, int 
           for (int n = 0; n < j.Cout; ++n) {
             const int64_t o = (raw_b - raw.data()) + (((int64_t)yo * j.raw_Cq + (n >> 2)) * j.raw_Wp + xo) * 4 + (n & 3);
             if (o < 0 || o >= (int64_t)raw.size()) { set_error("raw OOB"); return 7; }
-            const double v = acc[(size_t)m * Npad + n];
+            const double v = acc[(size_t)m * Npad + n] * j.w_unscale;
             raw[o] = v;
             written[o]++;
             for (int q = 0; q < 2; ++q) {
