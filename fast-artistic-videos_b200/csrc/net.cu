@@ -13,6 +13,7 @@
 #include <cmath>
 #include <cstring>
 
+#include "arena_plan.hpp"
 #include "conv_plan.hpp"
 
 namespace fav {
@@ -34,6 +35,7 @@ int launch_temporal_stage_structure(const float *content, const float *prev, con
                                     float *cert_out, const Operand &dst, int R, int H, int W, int r, int border_mode, cudaStream_t st);
 int launch_compute_corners(const float *image, float scale, int Z, int W, int H, float rho, float *corners, float *avg_out,
                            void *workspace, cudaStream_t st);
+int launch_clear_border(const Operand &o, int nimg, cudaStream_t st);
 int launch_image_scale_bicubic(const float *in, float *out, int C, int Hin, int Win, int Hout, int Wout, cudaStream_t st);
 int check_scale_args(const float *in, const float *out, int C, int Hin, int Win, int Hout, int Wout);
 
@@ -86,16 +88,24 @@ struct PlanStep {
   int raw_sel = 0;       // raw.p is Plan::raw_buf (0) or raw_buf2 (1)
   int layer_index = -1;  // arch token index whose output this step completes (for fav_net_layer_output)
   bool fused_nl = false; // kind 1: the tensor-core consumer normalises on load (conv_tc.cu), this pass is skipped
+  int clear = -1;        // arena plans: the operand this step writes first, whose border it zeroes before it runs
 };
 
 // a batch: B frames of one size run through one plan, every kernel covering all B images in one launch (conv.cuh tile_at);
 // operands, raw tensors and statistics hold one image after the other, each with its own zero border
 constexpr int kMaxBatch = 64;
-constexpr size_t kMaxPlanBytes = (size_t)32 << 30;  // activation buffers of one plan, checked before each allocation
+constexpr size_t kMaxPlanBytes = (size_t)32 << 30;  // default activation budget of one plan (fav_net_set_activation_budget)
 
 struct Plan {
   int B = 1, H = 0, W = 0;
-  size_t bytes = 0;        // device memory of the activation buffers (kMaxPlanBytes)
+  size_t bytes = 0;        // device memory of the activation buffers, checked against budget before each allocation
+  size_t budget = kMaxPlanBytes;
+  bool dry = false;        // sizes only: alloc_zero counts bytes and allocates nothing (build_plan's first pass)
+  // arena plan (arena_plan.hpp): operands share one buffer by lifetime.  preset: the hi / lo pointers make_operand hands out
+  // (null: its own buffer); kept: per operand, whether its bytes are intact after the frame (fav_net_layer_output)
+  void *arena = nullptr;
+  std::vector<std::pair<__half *, __half *>> preset;
+  std::vector<char> kept;
   int64_t stats_img = 0;   // doubles of statistics per image
   std::vector<Operand> ops;
   std::vector<void *> allocs;
@@ -148,6 +158,7 @@ struct fav_net {
   int device = 0;
   std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>> plans;  // (B, H, W)
   Plan *last_plan = nullptr;
+  size_t budget = kMaxPlanBytes;  // activation bytes of plans created from now on (fav_net_set_activation_budget)
   std::vector<void *> allocs;
   ~fav_net() {
     plans.clear();
@@ -313,9 +324,10 @@ static int fold_batch_norms(fav_net *net, std::vector<std::vector<float>> &w, st
 // ---- plan ---------------------------------------------------------------------------------------------------
 static int alloc_zero(Plan &pl, void **out, size_t bytes) {
   pl.bytes += bytes;
-  if (pl.bytes > kMaxPlanBytes) {
-    set_error("a batch of %d frames of %dx%d needs more than %zu GiB of activations: use a smaller batch", pl.B, pl.W, pl.H,
-              kMaxPlanBytes >> 30);
+  if (pl.dry) { *out = nullptr; return FAV_OK; }
+  if (pl.bytes > pl.budget) {
+    set_error("a batch of %d frames of %dx%d needs more than %.2f GiB of activations (the activation budget, "
+              "fav_net_set_activation_budget): use a smaller batch", pl.B, pl.W, pl.H, pl.budget / 1073741824.0);
     return FAV_ERR_INVALID;
   }
   FAV_TRY(check_cuda(cudaMalloc(out, bytes), "cudaMalloc(activations)"));
@@ -327,8 +339,13 @@ static int alloc_zero(Plan &pl, void **out, size_t bytes) {
 static int make_operand(Plan &pl, int C, int H, int W, const ConvDef *consumer, int *index) {
   Operand o = operand_geometry(C, H, W, consumer);
   o.img16 = (int64_t)o.elems16;
-  FAV_TRY(alloc_zero(pl, (void **)&o.hi, pl.B * o.elems16 * 16));
-  FAV_TRY(alloc_zero(pl, (void **)&o.lo, pl.B * o.elems16 * 16));
+  const size_t i = pl.ops.size();
+  if (i < pl.preset.size() && pl.preset[i].first) {
+    o.hi = pl.preset[i].first; o.lo = pl.preset[i].second;
+  } else {
+    FAV_TRY(alloc_zero(pl, (void **)&o.hi, pl.B * o.elems16 * 16));
+    FAV_TRY(alloc_zero(pl, (void **)&o.lo, pl.B * o.elems16 * 16));
+  }
   pl.ops.push_back(o);
   *index = (int)pl.ops.size() - 1;
   return FAV_OK;
@@ -428,21 +445,9 @@ static void fuse_norm_on_load(fav_net *net, Plan &pl, PlanStep &cs, bool src_is_
   ap.fused_nl = true;
 }
 
-static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
-  if (B < 1 || B > kMaxBatch) {
-    set_error("batch of %d frames: 1 to %d frames per call", B, kMaxBatch);
-    return FAV_ERR_INVALID;
-  }
-  auto key = std::make_tuple(B, H, W);
-  auto it = net->plans.find(key);
-  if (it != net->plans.end()) { *out = it->second.get(); net->last_plan = *out; return FAV_OK; }
-  if (H % 4 || W % 4 || H < 16 || W < 16) {
-    set_error("frame size %dx%d: H and W must be multiples of 4 and at least 16 (the default arch's two stride-2 layers "
-              "restore the input size only then, SURVEY appendix B)", W, H);
-    return FAV_ERR_INVALID;
-  }
-  std::unique_ptr<Plan> pl(new Plan());
-  pl->B = B; pl->H = H; pl->W = W;
+// the buffers and steps of plan pl (B, H, W, budget, dry and preset set by the caller)
+static int build_plan_steps(fav_net *net, Plan *pl) {
+  const int B = pl->B, H = pl->H, W = pl->W;
   const int R = net->reflect_pad;
   if (R >= H || R >= W) { set_error("frame smaller than the reflection padding (%d)", R); return FAV_ERR_INVALID; }
   // pass 1: sizes -> largest raw tensor, stats slots
@@ -558,6 +563,97 @@ static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
       pl->steps.push_back(std::move(ns));
     }
   }
+  return FAV_OK;
+}
+
+// the plan's steps as the buffer planner sees them.  A batch-normalized net's conv epilogue writes the next operand (and reads
+// the skip) itself; the norm step after it does the same on the CUDA-core comparator.
+static std::vector<ArenaStep> arena_steps(const fav_net *net, const Plan &pl) {
+  std::vector<ArenaStep> v(pl.steps.size());
+  for (size_t si = 0; si < pl.steps.size(); ++si) {
+    const PlanStep &s = pl.steps[si];
+    ArenaStep &a = v[si];
+    if (s.kind != 1) a.src = s.src;
+    if (s.kind != 0) { a.dst = s.dst; a.skip = s.skip; }
+    if (s.kind == 0 && net->bn && si + 1 < pl.steps.size() && pl.steps[si + 1].kind == 1) {
+      a.dst = pl.steps[si + 1].dst; a.skip = pl.steps[si + 1].skip;
+    }
+  }
+  return v;
+}
+
+// The activation bytes of a (B, H, W) plan with every operand in its own buffer (all_live) and with the operands in one arena
+// (arena_plan.hpp; *ap, when given, receives the arena layout).  The network's first operand stays out of the arena: the
+// temporal-stage kernels write it before the frame's steps run, and fav_net_layer_output's replay starts from it.
+static int plan_sizes(fav_net *net, int B, int H, int W, size_t *all_live, size_t *arena, ArenaPlan *ap = nullptr) {
+  Plan dry;
+  dry.B = B; dry.H = H; dry.W = W; dry.dry = true;
+  FAV_TRY(build_plan_steps(net, &dry));
+  std::vector<size_t> bytes(dry.ops.size());
+  std::vector<char> pinned(dry.ops.size(), 0);
+  size_t own = 0;  // what the arena operands take in buffers of their own
+  for (size_t i = 0; i < dry.ops.size(); ++i) {
+    const size_t half = (size_t)B * dry.ops[i].elems16 * 16;  // hi, then lo at the next kArenaAlign boundary
+    bytes[i] = 2 * ((half + kArenaAlign - 1) / kArenaAlign * kArenaAlign);
+    if (i) own += 2 * half;
+  }
+  pinned[0] = 1;
+  ArenaPlan p = plan_arena(arena_steps(net, dry), bytes, pinned);
+  *all_live = dry.bytes;
+  *arena = dry.bytes - own + p.arena_bytes;
+  if (ap) *ap = std::move(p);
+  return FAV_OK;
+}
+
+// A plan whose buffers fit the net's activation budget each get their own (zeroed once).  Otherwise the operands share one
+// arena by lifetime; each step that writes an operand first zeroes its border (launch_clear_border).  The choice depends on
+// (B, H, W) and the budget only.
+static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
+  if (B < 1 || B > kMaxBatch) {
+    set_error("batch of %d frames: 1 to %d frames per call", B, kMaxBatch);
+    return FAV_ERR_INVALID;
+  }
+  auto key = std::make_tuple(B, H, W);
+  auto it = net->plans.find(key);
+  if (it != net->plans.end()) { *out = it->second.get(); net->last_plan = *out; return FAV_OK; }
+  if (H % 4 || W % 4 || H < 16 || W < 16) {
+    set_error("frame size %dx%d: H and W must be multiples of 4 and at least 16 (the default arch's two stride-2 layers "
+              "restore the input size only then, SURVEY appendix B)", W, H);
+    return FAV_ERR_INVALID;
+  }
+  size_t all_live = 0, shared = 0;
+  ArenaPlan ap;
+  FAV_TRY(plan_sizes(net, B, H, W, &all_live, &shared, &ap));
+  std::unique_ptr<Plan> pl(new Plan());
+  pl->B = B; pl->H = H; pl->W = W; pl->budget = net->budget;
+  if (all_live > net->budget) {
+    if (shared > net->budget) {
+      set_error("a batch of %d frames of %dx%d needs %.2f GiB of activations, %.2f GiB with buffers shared between layers; the "
+                "activation budget is %.2f GiB (fav_net_set_activation_budget): use a smaller batch", B, W, H,
+                all_live / 1073741824.0, shared / 1073741824.0, net->budget / 1073741824.0);
+      return FAV_ERR_INVALID;
+    }
+    FAV_TRY(check_cuda(cudaMalloc(&pl->arena, ap.arena_bytes), "cudaMalloc(activation arena)"));
+    pl->allocs.push_back(pl->arena);
+    pl->bytes += ap.arena_bytes;
+    // no operand may rely on what the arena held before its producer ran: fill it with fp16 NaNs, not zeros
+    FAV_TRY(check_cuda(cudaMemset(pl->arena, 0xff, ap.arena_bytes), "cudaMemset(activation arena)"));
+    pl->preset.assign(ap.off.size(), {nullptr, nullptr});
+    for (size_t i = 0; i < ap.off.size(); ++i) {
+      if (ap.first[i] < 0) continue;
+      char *hi = (char *)pl->arena + ap.off[i];
+      pl->preset[i] = {(__half *)hi, (__half *)(hi + ap.bytes[i] / 2)};  // hi, then lo
+    }
+    pl->kept = ap.kept;
+  }
+  FAV_TRY(build_plan_steps(net, pl.get()));
+  if (pl->arena) {
+    for (size_t i = 0; i < pl->ops.size(); ++i) {
+      if (ap.first[i] < 0) continue;
+      if (pl->steps[ap.first[i]].clear >= 0) { set_error("internal: two operands become live at step %d", ap.first[i]); return FAV_ERR_INVALID; }
+      pl->steps[ap.first[i]].clear = (int)i;
+    }
+  }
   *out = pl.get();
   net->last_plan = pl.get();
   net->plans[key] = std::move(pl);
@@ -614,6 +710,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
   }
   for (size_t si = 0; si < pl.steps.size() && (last < 0 || (int)si <= last); ++si) {
     PlanStep &s = pl.steps[si];
+    if (s.clear >= 0) FAV_TRY(launch_clear_border(pl.ops[s.clear], pl.B, st));
     if (s.kind == 0) {
       {
         const ConvDef &c = net->convs[s.conv];
@@ -910,6 +1007,21 @@ int fav_net_set_conv_impl(fav_net_t *net, int impl) {
   return FAV_OK;
 }
 
+int fav_net_set_activation_budget(fav_net_t *net, size_t bytes) {
+  FAV_REQUIRE(net && bytes > 0, "fav_net_set_activation_budget: null net or zero budget");
+  net->budget = bytes;
+  return FAV_OK;
+}
+
+int fav_net_plan_bytes(fav_net_t *net, int B, int H, int W, size_t *all_live, size_t *shared) {
+  FAV_REQUIRE(net && all_live && shared, "fav_net_plan_bytes: null argument");
+  FAV_REQUIRE(net->finalized, "fav_net_plan_bytes: call fav_net_finalize first");
+  FAV_REQUIRE(B >= 1 && B <= kMaxBatch, "batch of %d frames: 1 to %d frames per call", B, kMaxBatch);
+  FAV_REQUIRE(H % 4 == 0 && W % 4 == 0 && H >= 16 && W >= 16, "frame size %dx%d: H and W must be multiples of 4 and at least 16",
+              W, H);
+  return plan_sizes(net, B, H, W, all_live, shared);
+}
+
 int fav_net_forward(fav_net_t *net, const float *in7, int H, int W, float *out3, void *stream) {
   return fav_net_forward_batch(net, in7, 1, H, W, out3, stream);
 }
@@ -958,6 +1070,12 @@ int fav_net_layer_output_image(fav_net_t *net, int index, int b, float *out, int
   auto it = pl->layer_operand.find(index);
   FAV_REQUIRE(it != pl->layer_operand.end(), "fav_net_layer_output: layer %d has no stored activation", index);
   const Operand &o = pl->ops[it->second];
+  if (pl->arena) {  // operands share buffers: a later layer may have taken this one over, and a replay would clobber others
+    bool fused = false;
+    for (const PlanStep &s : pl->steps) fused |= s.layer_index == index && s.kind == 1 && s.fused_nl && net->conv_impl == 0;
+    FAV_REQUIRE(pl->kept[it->second] && !fused, "fav_net_layer_output: layer %d of the %dx%d plan (batch of %d) is not kept: "
+                "its activations share buffers with later layers (fav_net_set_activation_budget)", index, pl->W, pl->H, pl->B);
+  }
   if (C) *C = o.C;
   if (Hl) *Hl = o.H;
   if (Wl) *Wl = o.W;

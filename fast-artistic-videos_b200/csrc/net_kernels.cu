@@ -3,6 +3,7 @@
 //   in_stats        : per-channel sum / sum of squares of a raw conv output         InstanceNormalization.lua:33-53
 //   in_finalize     : mean, gamma/sqrt(var+eps), beta (biased variance, eps 1e-5)
 //   in_apply        : normalise (+ReLU) (+ShaveImage(2) skip add) -> next operand    models_video.lua:41-53,121-130
+//   clear_border    : zero an operand's border before its producer runs (operands sharing an arena, arena_plan.hpp)
 //   unpack_operand  : operand -> fp32 NCHW (per-layer parity checks)
 //   conv_simt       : direct convolution on CUDA cores, same I/O as the tcgen05 kernel (bring-up comparator)
 #include "conv.cuh"
@@ -294,6 +295,50 @@ int launch_up_in(const Operand &src, double *sums, const float *gamma, const flo
   up_apply_kernel<<<grid, 128, 0, st>>>(src, sums, gamma, beta, 1.0 / ((double)src.H * src.W), (double)eps, relu, scale, dst,
                                         tab_mean, tab_scale, sums_img);
   return post_launch("up_in.apply");
+}
+
+// ---- clear_border --------------------------------------------------------------------------------------------
+// Zero every 16-byte unit of an operand except its interior pixels: the border rows, the columns left of padL and right of
+// padL + W (row slack included), both planes of a parity-split slab, and the tail slack -- everything operand_geometry gives
+// its readers beyond what in_apply, up_apply and the operand epilogue write.  An operand in a shared arena (arena_plan.hpp)
+// holds its previous occupant's data there until this runs.  One warp per storage row of one channel block; interior rows
+// clear their (Ws - W)-odd units only.  Batch: blockIdx.y = image.
+constexpr int kClearWarps = 8;
+
+__global__ void __launch_bounds__(32 * kClearWarps) clear_border_kernel(Operand o) {
+  o = image_of(o, blockIdx.y);
+  uint4 *hi = reinterpret_cast<uint4 *>(o.hi), *lo = reinterpret_cast<uint4 *>(o.lo);
+  const uint4 z = make_uint4(0, 0, 0, 0);
+  const int lane = threadIdx.x & 31;
+  const int64_t slab = o.slab16(), rows = (int64_t)o.Hs * o.Cb;
+  const int64_t row = (int64_t)blockIdx.x * kClearWarps + (threadIdx.x >> 5);
+  if (row == rows) {  // tail slack
+    for (int64_t i = rows * slab + lane; i < (int64_t)o.elems16; i += 32) { hi[i] = z; lo[i] = z; }
+    return;
+  }
+  if (row > rows) return;
+  const int ys = (int)(row / o.Cb);
+  const int64_t base = row * slab;
+  if (ys < o.padT || ys >= o.padT + o.H) {
+    for (int64_t i = lane; i < slab; i += 32) { hi[base + i] = z; lo[base + i] = z; }
+    return;
+  }
+  // plane p (parity split: x = 2 j + p) holds interior pixels at slots [lo_p, hi_p) of its pw slots
+  const int np = o.parity ? 2 : 1, pw = o.parity ? o.Ws2 : o.Ws;
+  for (int p = 0; p < np; ++p) {
+    const int a = o.parity ? (o.padL - p + 1) >> 1 : o.padL, b = o.parity ? (o.padL + o.W - p + 1) >> 1 : o.padL + o.W;
+    const int n = pw - (b - a);
+    for (int k = lane; k < n; k += 32) {
+      const int64_t i = base + (int64_t)p * pw + (k < a ? k : b + (k - a));
+      hi[i] = z; lo[i] = z;
+    }
+  }
+}
+
+int launch_clear_border(const Operand &o, int nimg, cudaStream_t st) {
+  const int64_t rows = (int64_t)o.Hs * o.Cb + 1;  // + the tail
+  clear_border_kernel<<<dim3((unsigned)ceil_div64(rows, kClearWarps), nimg), 32 * kClearWarps, 0, st>>>(o);
+  return post_launch("clear_border");
 }
 
 // ---- unpack_operand (debug) -----------------------------------------------------------------------------

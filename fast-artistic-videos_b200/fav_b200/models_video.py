@@ -67,6 +67,18 @@ class StyleNet:
         """'tcgen05' (default) or 'simt' (CUDA-core comparator used for bring-up / debugging)."""
         _lib.check(_lib.lib.fav_net_set_conv_impl(self._h, {"tcgen05": 0, "simt": 1}[impl]))
 
+    def set_activation_budget(self, nbytes: int) -> None:
+        """Cap the activation memory of plans (one per batch and frame size) created from now on; default 32 GiB.  A plan
+        over the budget shares buffers between layers whose lifetimes do not overlap (same output, bit for bit); one over
+        it even then is refused (FavError)."""
+        _lib.check(_lib.lib.fav_net_set_activation_budget(self._h, int(nbytes)))
+
+    def plan_bytes(self, H: int, W: int, batch: int = 1):
+        """(all-live bytes, shared-arena bytes) of the activation buffers a plan for `batch` frames of H x W takes."""
+        a, s = C.c_size_t(), C.c_size_t()
+        _lib.check(_lib.lib.fav_net_plan_bytes(self._h, int(batch), int(H), int(W), C.byref(a), C.byref(s)))
+        return a.value, s.value
+
     # -- model:forward(input) ----------------------------------------------------------------------
     def forward(self, input: torch.Tensor) -> torch.Tensor:
         assert input.dim() == 4 and input.size(0) >= 1 and input.size(1) == self.in_dim, \

@@ -225,13 +225,27 @@ FAV_API int fav_net_layer_output(fav_net_t *net, int index, float *out, int *C, 
  * train_video.lua:60 trains with -batch_size 4).  The *_batch calls take B frames of one size stored one after the other and run
  * them through one plan: every kernel covers all B images in one launch, and a run_* call is still ONE graph launch.  Image b of
  * a batch is bit-identical to the same frame run alone.  B = 1 is the single-frame call.  FAV_ERR_INVALID for B < 1, B > 64, or
- * a batch whose activation buffers would exceed 32 GiB (checked before they are allocated).
+ * a batch whose activation buffers would exceed the activation budget even when shared (fav_net_set_activation_budget, checked
+ * before they are allocated).
  *
  * model:forward(input) of a batch                fast_artistic_video_core.lua:138,172
  * in [B,in_dim,H,W] device fp32 -> out3 [B,3,H,W] device fp32 in net space. */
 FAV_API int fav_net_forward_batch(fav_net_t *net, const float *in, int B, int H, int W, float *out3, void *stream);
 /* fav_net_layer_output for image b of the last forward's batch (models_video.lua:55-140 layer `index`). */
 FAV_API int fav_net_layer_output_image(fav_net_t *net, int index, int b, float *out, int *C, int *Hl, int *Wl, void *stream);
+
+/* Activation memory.  A plan (one per batch size B and frame size H x W, built at its first call) gives every activation its
+ * own buffer when their total fits the net's activation budget.  When it does not, activations whose lifetimes do not overlap
+ * share one arena, and the kernels and their order stay the same: the output is bit-identical to the all-live plan's.  On
+ * such a plan fav_net_layer_output returns FAV_ERR_INVALID for a layer whose activation a later layer has taken over (the
+ * input of the final layer stays readable).  A plan whose shared arena exceeds the budget as well is refused with
+ * FAV_ERR_INVALID, both figures in the message.
+ *
+ * The budget applies to plans created after the call; plans already built keep their buffers.  Default: 32 GiB. */
+FAV_API int fav_net_set_activation_budget(fav_net_t *net, size_t bytes);
+/* The activation bytes a (B, H, W) plan takes with every activation in its own buffer (*all_live) and with buffers shared by
+ * lifetime (*shared), without allocating anything.  After fav_net_finalize. */
+FAV_API int fav_net_plan_bytes(fav_net_t *net, int B, int H, int W, size_t *all_live, size_t *shared);
 
 /* ---------------------------------------------------------------------------------------------
  * f-5  the perceptual loss network of -evaluate: nn.PerceptualCriterion with nn.ContentLoss / nn.StyleLoss
