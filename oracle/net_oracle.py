@@ -68,42 +68,62 @@ class NetOracle:
             return self.operand_round(x, wt, b, kw, True)
         return F.conv_transpose2d(x, wt, b, **kw)
 
+    def to(self, device) -> "NetOracle":
+        """Moves the weights to `device` (e.g. "cuda": cuDNN in fp64 for frames a CPU forward cannot reach); layer and forward
+        then take inputs on that device."""
+        self.w = {k: v.to(device) for k, v in self.w.items()}
+        return self
+
+    def layer(self, i: int, x: torch.Tensor, norm_hook=None) -> torch.Tensor:
+        """Arch token i's step on x, the output of step i - 1 (for i = 0 the 1xCxHxW net input, which the reflect-start
+        padding then pads): conv / transposed conv / nearest upsample / residual block, then InstanceNorm and ReLU.
+        norm_hook(name, t): optional, called with the input t of each InstanceNorm the step runs."""
+        s, n = self.specs[i], f"l{i}"
+        x = x.to(self.dtype)
+
+        def inorm(t, name):
+            if norm_hook is not None:
+                norm_hook(name, t)
+            return _inorm(t, self.w, name)
+
+        if i == 0 and self.pad:
+            x = F.pad(x, (self.pad,) * 4, mode="reflect")  # train_video.lua:322
+        if s["kind"] == "conv":
+            x = self._conv(x, n, s["stride"], s["pad"])
+        elif s["kind"] == "fullconv":
+            x = self._fullconv(x, n, s)
+        elif s["kind"] == "up":
+            x = F.interpolate(x, scale_factor=s["scale"], mode="nearest")
+        elif s["kind"] == "res":  # build_conv_block :10-39 (+ ConcatTable / CAddTable :41-53 for RX)
+            bp = self.block_pad
+            y = self._conv(x, n + ".c1", 1, bp)
+            y = torch.relu(inorm(y, n + ".n1"))
+            y = self._conv(y, n + ".c2", 1, bp)
+            y = inorm(y, n + ".n2")
+            if not s.get("skip", True):
+                x = y                                    # CX
+            elif bp:
+                x = y + x                                # Identity skip ('zero')
+            else:
+                x = y + x[:, :, 2:-2, 2:-2]              # ShaveImage(2) + CAddTable
+        if s["in_norm"]:
+            x = inorm(x, n + ".n")
+        if s["relu"]:
+            x = torch.relu(x)
+        return x
+
     def forward(self, x7: torch.Tensor, taps=None) -> torch.Tensor:
         """x7: 1x7xHxW -> 1x3xHxW (net space, before deprocess).  taps: optional dict to record activations."""
-        x = x7.to(self.dtype)
-        if self.pad:
-            x = F.pad(x, (self.pad,) * 4, mode="reflect")  # train_video.lua:322
-        for i, s in enumerate(self.specs):
-            n = f"l{i}"
-            if s["kind"] == "conv":
-                x = self._conv(x, n, s["stride"], s["pad"])
-            elif s["kind"] == "fullconv":
-                x = self._fullconv(x, n, s)
-            elif s["kind"] == "up":
-                x = F.interpolate(x, scale_factor=s["scale"], mode="nearest")
-            elif s["kind"] == "res":  # build_conv_block :10-39 (+ ConcatTable / CAddTable :41-53 for RX)
-                bp = self.block_pad
-                y = self._conv(x, n + ".c1", 1, bp)
-                y = torch.relu(_inorm(y, self.w, n + ".n1"))
-                y = self._conv(y, n + ".c2", 1, bp)
-                y = _inorm(y, self.w, n + ".n2")
-                if not s.get("skip", True):
-                    x = y                                    # CX
-                elif bp:
-                    x = y + x                                # Identity skip ('zero')
-                else:
-                    x = y + x[:, :, 2:-2, 2:-2]              # ShaveImage(2) + CAddTable
-            if s["in_norm"]:
-                x = _inorm(x, self.w, n + ".n")
-            if s["relu"]:
-                x = torch.relu(x)
+        x = x7
+        for i in range(len(self.specs)):
+            x = self.layer(i, x)
             if taps is not None:
-                taps[n] = x
+                taps[f"l{i}"] = x
         return torch.tanh(x) * self.tanh_constant  # models_video.lua:135-136
 
     # --- frame-level restatements -----------------------------------------------------------
     def deprocess(self, y):  # preprocess.lua:66-71
-        mean = torch.tensor(VGG_MEAN, dtype=self.dtype).view(1, 3, 1, 1)
+        mean = torch.tensor(VGG_MEAN, dtype=self.dtype, device=y.device).view(1, 3, 1, 1)
         return ((y + mean) / 255.0)[:, [2, 1, 0]]
 
     def run_image(self, content01: np.ndarray) -> np.ndarray:

@@ -145,3 +145,24 @@ def test_net_oracle_structure():
     # appendix B size rule: 48x64 -> 128x144 -> 64x72 -> 32x36 -> (5 res) 12x16 -> 24x32 -> 48x64
     assert tuple(taps["l0"].shape[-2:]) == (128, 144) and tuple(taps["l2"].shape[-2:]) == (32, 36)
     assert tuple(taps["l7"].shape[-2:]) == (12, 16) and tuple(taps["l9"].shape[-2:]) == (48, 64)
+
+
+@pytest.mark.parametrize("ptype", ["reflect-start", "zero"])
+@pytest.mark.parametrize("arch", [synth.DEFAULT_ARCH, synth.PAPER_ARCH], ids=["default", "paper"])
+def test_net_oracle_forward_is_the_chained_layers(arch, ptype):
+    """forward == layer(0) -> layer(1) -> ... -> tanh * 150, bit for bit: the GPU tests that feed each layer the product's own
+    previous activation (teacher forcing) check against exactly the steps the free-running oracle takes."""
+    net = net_oracle.NetOracle(arch=arch, padding_type=ptype)
+    rng = np.random.default_rng(3)
+    x7 = torch.from_numpy(rng.normal(0, 50, (1, 7, 64, 96)))
+    taps = {}
+    ref = net.forward(x7, taps)
+    x = x7
+    for i in range(len(net.specs)):
+        x = net.layer(i, x)
+        assert torch.equal(x, taps[f"l{i}"]), f"layer {i}"
+    assert torch.equal(torch.tanh(x) * net.tanh_constant, ref)
+    seen = []
+    net.layer(3, taps["l2"], norm_hook=lambda name, t: seen.append((name, tuple(t.shape[1:]))))
+    shapes = [(128, 34, 42), (128, 32, 40)] if ptype == "reflect-start" else [(128, 16, 24)] * 2  # 36x44 in, pad-0 convs
+    assert seen == list(zip(["l3.n1", "l3.n2"], shapes)), seen
