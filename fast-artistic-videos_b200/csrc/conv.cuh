@@ -124,7 +124,24 @@ struct ConvJob {
   // the weights are packed multiplied by 2^w_exp (ConvDef::w_exp): every epilogue takes acc * w_unscale = acc * 2^-w_exp before
   // the bias.  The operand epilogue has it folded into epi_scale instead.
   float w_unscale;
+  // precision (fav_net_set_precision): 0 = the fp16 pair, three MMAs per K step (hi*hi + lo*hi + hi*lo); 1 = single pass, one
+  // MMA per K step on the hi halves alone.  The operands and weights are the same; a single-pass launch copies and reads only
+  // their hi planes (the lo halves of the stages and weight slots go unused).  Picks the conv_tc_kernel instance.
+  int single;
 };
+
+// Bytes conv_tc_kernel's producers announce on a full barrier (mbarrier expect-tx): they must equal what the bulk copies land
+// there, or the barrier never completes.  Shared with the CPU emulator (tests/emu/fp16_mode_emu.cu).  pair == false: the
+// hi planes only.  A: one patch stage of the bulk-copy producer (not norm-on-load); B: one weight chunk, whose hi steps are
+// its first half ([hi steps][lo steps], pack_phase_weights).  dbg 4 / 2: the 16-byte timing ablations.
+__host__ __device__ inline uint32_t tc_a_stage_tx(const ConvJob &j, bool pair) {
+  uint32_t tx = 0;
+  for (int s = 0; s < j.nseg; ++s) tx += (j.dbg & 4) ? 16u : (uint32_t)j.seg_len16[s] * 16u;
+  return tx * (uint32_t)(j.nrows * j.CbG * (pair ? 2 : 1));
+}
+// chunk_bytes: ConvJob::chunk16 * 16, the whole chunk.  A macro: the same expression written as an inline function call changes
+// the register allocation of the pair instances (ptxas, CUDA 12.9), whose code stays as it was before the single pass.
+#define FAV_TC_B_CHUNK_TX(dbg, chunk_bytes, pair) (((dbg) & 2) ? 16u : ((pair) ? (chunk_bytes) : (chunk_bytes) / 2))
 
 // Tile T of a batched job, T = b * ntiles + t for image b and tile t of that image's output (0 <= T < nimg * ntiles): every role
 // of conv_tc_kernel (consumers, patch / weight / norm-on-load producers) walks T = blockIdx.x, blockIdx.x + gridDim.x, ... and

@@ -9,6 +9,8 @@
 // (measured 1.2e-3..2.7e-3, DESIGN.md §precision), so every operand is an fp16 pair x = hi + lo and each
 // K step issues three MMAs  hi*hi + lo*hi + hi*lo  (fp32 accumulation): ~2^-21 relative error while |x| >= 2^-3, which the
 // weights get from a power-of-two prescale undone in the epilogue (ConvJob::w_unscale, DESIGN.md §2).
+// The opt-in single pass (ConvJob::single, fav_net_set_precision "fp16"; template flag PAIR == false) issues hi*hi alone and
+// copies only the hi planes of the patch and of each weight chunk: fp16 operands, fp32 accumulation.
 //
 // Data movement: the input patch of a tile (all filter rows x a group of channel blocks x 128+halo pixels)
 // is fetched ONCE per tile by 1-D bulk async copies (cp.async.bulk, completion on an mbarrier).  Because the
@@ -112,7 +114,8 @@ __device__ __forceinline__ void tc_stats_add(float *slot, int warp, int lane, in
 // OPND: operand epilogue of batch-normalized nets (ConvJob::opnd) -- a template parameter, so the raw-output instances keep
 // their code and registers.  BATCH: nimg > 1.  The same code; BATCH == false compiles it with nimg == 1 (one image, every
 // image offset zero), so a single-frame launch keeps the code of a kernel without batches (about 1.5 % of a 720p frame).
-template <int NT, bool OPND, bool BATCH>
+// PAIR: the fp16 pair's three MMAs per K step; false: the single pass (ConvJob::single), hi * hi only.
+template <int NT, bool OPND, bool BATCH, bool PAIR>
 __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, uint8_t *b_base, TcShared *sh, float *exch) {
   constexpr int NJ = NT / 8;
   const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -154,8 +157,10 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
             const uint64_t ad_hi = kDescHi | (a_hi16 + dls), ad_lo = kDescHi | (a_lo16 + dls);
             const uint64_t bd_hi = kDescHi | bs, bd_lo = kDescHi | (bs + b_lo16);
             Wgmma<NT>::mma(acc, ad_hi, bd_hi, scale);
-            Wgmma<NT>::mma(acc, ad_lo, bd_hi, 1u);
-            Wgmma<NT>::mma(acc, ad_hi, bd_lo, 1u);
+            if constexpr (PAIR) {
+              Wgmma<NT>::mma(acc, ad_lo, bd_hi, 1u);
+              Wgmma<NT>::mma(acc, ad_hi, bd_lo, 1u);
+            }
             scale = 1;
           }
           wgmma_commit();
@@ -320,7 +325,7 @@ __device__ __forceinline__ void nl_build_table(const ConvJob &job, float *nl_tab
   }
 }
 
-template <int NT, bool OPND, bool BATCH>
+template <int NT, bool OPND, bool BATCH, bool PAIR>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ ConvJob job) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t a_stage_bytes = (uint32_t)job.stage16 * 16u;  // one of hi / lo
@@ -359,9 +364,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   const int ngroups = job.ngroups, nchunks = job.nchunks;
 
   if (warp < 8) {
-    tc_consume<NT, OPND, BATCH>(job, a_base, b_base, sh, exch);
+    tc_consume<NT, OPND, BATCH, PAIR>(job, a_base, b_base, sh, exch);
   } else if (job.nl && warp >= kAWarp) {
-    // ===== norm-on-load patch producers: raw fp32 -> InstanceNorm (+ReLU) -> fp16 hi/lo -> MMA-ready stage =====
+    // ===== norm-on-load patch producers: raw fp32 -> InstanceNorm (+ReLU) -> fp16 hi/lo -> MMA-ready stage (hi only: !PAIR) =====
     // The warps take turns over units of 32 kNlPx pixels of one (patch row, channel block) slab: lanes run along the slab,
     // kNlPx float4 pairs in flight per lane.  Units rather than whole slabs keep the warps evenly loaded when a slab is longer
     // than one unit (the 257 pixels of a stride-2 consumer).
@@ -423,7 +428,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
 #pragma unroll
               for (int i = 0; i < 4; ++i) split_pair(v[2 * i], v[2 * i + 1], h[i], l[i]);
               *reinterpret_cast<uint4 *>(drow + (uint32_t)p * 16u) = make_uint4(h[0], h[1], h[2], h[3]);
-              *reinterpret_cast<uint4 *>(drow + a_stage_bytes + (uint32_t)p * 16u) = make_uint4(l[0], l[1], l[2], l[3]);
+              if constexpr (PAIR)
+                *reinterpret_cast<uint4 *>(drow + a_stage_bytes + (uint32_t)p * 16u) = make_uint4(l[0], l[1], l[2], l[3]);
             }
           }
         }
@@ -435,12 +441,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     }
   } else if (warp == kAWarp) {
     // ===== A producer: the input patch of each (tile, channel group): one bulk copy per (patch row, channel block, hi/lo),
-    // spread over the 32 lanes =====
-    const int per_row = job.CbG * job.nseg * 2;  // copies per patch row (x2: hi, lo)
+    // spread over the 32 lanes (hi only: !PAIR) =====
+    constexpr int NP = PAIR ? 2 : 1;              // planes copied
+    const int per_row = job.CbG * job.nseg * NP;  // copies per patch row
     const int ncopies = job.nrows * per_row;
-    uint32_t stage_tx = 0;
-    for (int s = 0; s < job.nseg; ++s) stage_tx += (job.dbg & 4) ? 16u : (uint32_t)job.seg_len16[s] * 16u;
-    stage_tx *= (uint32_t)(job.nrows * job.CbG * 2);
+    const uint32_t stage_tx = tc_a_stage_tx(job, PAIR);
     uint32_t s = 0, ph = 0;
     for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
       const TileAt at = tile_at(job, tile, BATCH);
@@ -452,9 +457,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         uint8_t *stage = a_base + s * 2 * a_stage_bytes;
         for (int c = lane; c < ncopies; c += 32) {
           int ri = c / per_row, r = c - ri * per_row;
-          int cbi = r / (job.nseg * 2);
-          r -= cbi * job.nseg * 2;
-          int seg = r >> 1, part = r & 1;
+          int cbi = r / (job.nseg * NP);
+          r -= cbi * job.nseg * NP;
+          int seg = PAIR ? r >> 1 : r, part = PAIR ? r & 1 : 0;
           int64_t src16 = ((int64_t)(job.row_mul * y + job.grp_row[g][ri]) * job.a_Cb + job.grp_cb0[g] + cbi) *
                               job.a_slab16 + job.seg_src16[seg] + x0 + at.a16;
           const uint4 *src = (part ? job.a_lo : job.a_hi) + src16;
@@ -466,7 +471,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
       }
     }
   } else if (warp == kBWarp) {
-    // ===== B producer: weight chunks =====
+    // ===== B producer: weight chunks (the hi steps, the first half of each chunk, only: !PAIR) =====
     if (lane == 0) {
       uint32_t s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
@@ -474,7 +479,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         for (int g = 0; g < ngroups; ++g)
           for (int c = 0; c < nchunks; ++c) {
             mbar_wait(&sh->b_empty[s], ph ^ 1);
-            const uint32_t cb = (job.dbg & 2) ? 16u : chunk_bytes;
+            const uint32_t cb = FAV_TC_B_CHUNK_TX(job.dbg, chunk_bytes, PAIR);
             mbar_arrive_expect_tx(&sh->b_full[s], cb);
             bulk_g2s(b_base + s * chunk_bytes, job.b + (int64_t)(g * nchunks + c) * job.chunk16, cb, &sh->b_full[s]);
             if (++s == nslots) { s = 0; ph ^= 1; }
@@ -549,11 +554,13 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
     return FAV_ERR_UNSUPPORTED;
   }
   void (*kernel)(ConvJob) = nullptr;
-  const bool batch = job.nimg > 1;
+  const bool batch = job.nimg > 1, pair = !job.single;
+#define FAV_TC_PICK(N, P)                                                                                      \
+  (job.opnd ? (batch ? conv_tc_kernel<N, true, true, P> : conv_tc_kernel<N, true, false, P>)                   \
+            : (batch ? conv_tc_kernel<N, false, true, P> : conv_tc_kernel<N, false, false, P>))
 #define FAV_TC_CASE(N)                                                                                         \
   case N:                                                                                                      \
-    kernel = job.opnd ? (batch ? conv_tc_kernel<N, true, true> : conv_tc_kernel<N, true, false>)              \
-                      : (batch ? conv_tc_kernel<N, false, true> : conv_tc_kernel<N, false, false>);           \
+    kernel = pair ? FAV_TC_PICK(N, true) : FAV_TC_PICK(N, false);                                              \
     break;
   switch (job.Npad) {
     FAV_TC_CASE(16) FAV_TC_CASE(32) FAV_TC_CASE(48) FAV_TC_CASE(64) FAV_TC_CASE(80) FAV_TC_CASE(96) FAV_TC_CASE(112)
@@ -563,6 +570,7 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
       return FAV_ERR_UNSUPPORTED;
   }
 #undef FAV_TC_CASE
+#undef FAV_TC_PICK
   // one persistent CTA per SM over the tiles of every image (tile_at); the grid of a single image is unchanged
   const int total = job.nimg * job.ntiles, grid = total < num_sms ? total : num_sms;
   job.trace = conv_trace_claim((size_t)grid * kTraceWords);
@@ -572,11 +580,11 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
     return FAV_ERR_UNSUPPORTED;
   }
   // the opt-in to > 48 KB of dynamic shared memory is a PER-DEVICE attribute of each instantiation
-  static std::atomic<uint64_t> attr_set[36];
+  static std::atomic<uint64_t> attr_set[72];
   int dev = 0;
   FAV_TRY(check_cuda(cudaGetDevice(&dev), "cudaGetDevice"));
   const uint64_t bit = 1ull << (dev & 63);
-  std::atomic<uint64_t> &set = attr_set[job.Npad / 16 + (job.opnd ? 9 : 0) + (batch ? 18 : 0)];
+  std::atomic<uint64_t> &set = attr_set[job.Npad / 16 + (job.opnd ? 9 : 0) + (batch ? 18 : 0) + (pair ? 0 : 36)];
   if (!(set.load(std::memory_order_acquire) & bit)) {
     FAV_TRY(check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
                        "cudaFuncSetAttribute(conv_tc)"));

@@ -153,6 +153,7 @@ struct fav_net {
   std::vector<SpecOp> ops;
   bool finalized = false;
   int conv_impl = 0;
+  int single = 0;  // fav_net_set_precision: 1 = "fp16", one MMA per K step (ConvJob::single); 0 = "pair"
   int num_sms = 148;
   cudaStream_t cap_stream = nullptr;  // graph capture happens here (the caller's stream may be the legacy default stream)
   int device = 0;
@@ -375,6 +376,7 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
           j.raw = raw; j.raw_Cq = st.raw.Cq; j.raw_Wp = st.raw.Wp;
           j.final_mode = 0; j.out3 = out3; j.tanh_c = net->tanh_c;
           conv_nblock_stats(j, stats, c.cout, b);
+          j.single = net->single;
           conv_tc_choose_slots(j);
           if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
           if (conv_tc_smem_bytes(j) > 227 * 1024) { set_error("conv %s: shared memory budget exceeded (fold)", c.name.c_str()); return FAV_ERR_UNSUPPORTED; }
@@ -390,6 +392,7 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
         conv_nblock_stats(j, stats, c.cout, b);
         if (epi)
           set_opnd_epilogue(j, b, cd.d_scale, pl.ops[epi->dst], epi->relu, epi->skip >= 0 ? &pl.ops[epi->skip] : nullptr, epi->shave);
+        j.single = net->single;  // the norm-on-load copies (fuse_norm_on_load) and tc_plain keep it
         conv_tc_choose_slots(j);
         if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
         if (conv_tc_smem_bytes(j) > 227 * 1024) {
@@ -1004,6 +1007,23 @@ int fav_net_finalize(fav_net_t *net) {
 int fav_net_set_conv_impl(fav_net_t *net, int impl) {
   FAV_REQUIRE(net && (impl == 0 || impl == 1), "fav_net_set_conv_impl: impl must be 0 (tcgen05) or 1 (CUDA cores)");
   net->conv_impl = impl;
+  return FAV_OK;
+}
+
+// The plans (and their CUDA graphs) hold jobs built for one precision: switching drops them, and the next call rebuilds.
+int fav_net_set_precision(fav_net_t *net, const char *mode) {
+  FAV_REQUIRE(net && mode, "fav_net_set_precision: null argument");
+  int single;
+  if (!strcmp(mode, "pair")) single = 0;
+  else if (!strcmp(mode, "fp16")) single = 1;
+  else {
+    set_error("fav_net_set_precision: mode \"%s\": \"pair\" (exact fp32 parity) or \"fp16\" (single pass)", mode);
+    return FAV_ERR_INVALID;
+  }
+  if (single == net->single) return FAV_OK;
+  net->plans.clear();
+  net->last_plan = nullptr;
+  net->single = single;
   return FAV_OK;
 }
 

@@ -82,6 +82,7 @@ SIGNATURES = {
     "fav_net_set_param": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
     "fav_net_finalize": (C.c_int, [C.c_void_p]),
     "fav_net_set_conv_impl": (C.c_int, [C.c_void_p, C.c_int]),
+    "fav_net_set_precision": (C.c_int, [C.c_void_p, C.c_char_p]),
     "fav_net_forward": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp, _fp]),
     "fav_net_profile": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_float),
                                   C.POINTER(C.c_double), C.c_char_p, C.POINTER(C.c_int), _fp]),

@@ -36,6 +36,15 @@ def _opt(opt, k, d=None):
     return opt.get(k, d) if isinstance(opt, dict) else getattr(opt, k, d)
 
 
+def set_precision(opt, *models) -> None:
+    """-precision pair|fp16 (an addition, StyleNet.set_precision) on every net the driver runs: the video model and the image
+    model, whichever driver (native pipeline, session, synchronous loop) then runs them."""
+    mode = _opt(opt, "precision", "pair")
+    for m in models:
+        if m is not None and getattr(m, "precision", "pair") != mode:
+            m.set_precision(mode)
+
+
 def load_model(path_or_style: str, arch: str = synth.DEFAULT_ARCH, in_dim: int = 7) -> models_video.StyleNet:
     """get_model (core.lua:38-57): a Torch7 `.t7` checkpoint (fav_b200/t7.py; the arch is recovered from the module
     tree), a `.npz` state dict, or `synthetic:<style>` = seeded random-init weights (no network here to fetch the
@@ -111,6 +120,7 @@ def run_fast_neural_video(opt, func_load_image, func_load_cert, func_eval, func_
     model_img = model_img if model_img is not None else (
         None if _opt(opt, "model_img", "self") in ("self", "", None)
         else load_model(_opt(opt, "model_img"), _opt(opt, "arch_img", _opt(opt, "arch", synth.DEFAULT_ARCH)), in_dim=3))
+    set_precision(opt, model, model_img)
     evaluate_image = make_evaluate_image(opt) if evaluate else None
     fill_mode = _opt(opt, "fill_occlusions", "vgg-mean")
     assert fill_mode in ("vgg-mean", "uniform-random")

@@ -20,9 +20,10 @@ from . import _lib, synth
 
 class StyleNet:
     def __init__(self, arch: str = synth.DEFAULT_ARCH, padding_type: str = "reflect-start",
-                 tanh_constant: float = 150.0, in_dim: int = 7, norm: str = "instance"):
+                 tanh_constant: float = 150.0, in_dim: int = 7, norm: str = "instance", precision: str = "pair"):
         """norm: 'instance' (InstanceNormalization, the default) or 'batch' (SpatialBatchNormalization in evaluate mode,
-        -use_instance_norm 0; its parameters add '<n>.running_mean', '<n>.running_var' and '<n>.eps')."""
+        -use_instance_norm 0; its parameters add '<n>.running_mean', '<n>.running_var' and '<n>.eps').
+        precision: 'pair' (fp32 parity, the default) or 'fp16' (single pass; set_precision)."""
         h = C.c_void_p()
         _lib.check(_lib.lib.fav_net_create_norm(arch.encode(), padding_type.encode(), C.c_float(tanh_constant), in_dim,
                                                 norm.encode(), C.byref(h)))
@@ -31,6 +32,9 @@ class StyleNet:
         self.in_dim = in_dim
         self.norm = norm
         self.finalized = False
+        self.precision = "pair"
+        if precision != "pair":
+            self.set_precision(precision)
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -66,6 +70,14 @@ class StyleNet:
     def set_conv_impl(self, impl: str) -> None:
         """'tcgen05' (default) or 'simt' (CUDA-core comparator used for bring-up / debugging)."""
         _lib.check(_lib.lib.fav_net_set_conv_impl(self._h, {"tcgen05": 0, "simt": 1}[impl]))
+
+    def set_precision(self, mode: str) -> None:
+        """'pair' (default): fp16 hi + lo operands, three MMAs per K step, fp32 parity.  'fp16': one MMA per K step on the hi
+        halves, faster, about one 8-bit level off the exact frame (fav_net_set_precision).  An addition, not a reference
+        option.  Drops the cached plans and graphs; frames in flight on a Session must be finished (Session.sync) first.
+        The CUDA-core comparator (set_conv_impl('simt')) stays exact fp32."""
+        _lib.check(_lib.lib.fav_net_set_precision(self._h, mode.encode()))
+        self.precision = mode
 
     def set_activation_budget(self, nbytes: int) -> None:
         """Cap the activation memory of plans (one per batch and frame size) created from now on; default 32 GiB.  A plan
@@ -216,10 +228,12 @@ def _planes(t, img, c):
 
 
 def build_model(opt) -> StyleNet:
-    """M.build_model(opt) (models_video.lua:55): opt.arch, opt.padding_type, opt.tanh_constant, opt.use_instance_norm."""
+    """M.build_model(opt) (models_video.lua:55): opt.arch, opt.padding_type, opt.tanh_constant, opt.use_instance_norm; and
+    opt.precision ('pair' or 'fp16', StyleNet.set_precision), an addition."""
     get = (lambda k, d: opt.get(k, d)) if isinstance(opt, dict) else (lambda k, d: getattr(opt, k, d))
     return StyleNet(get("arch", synth.DEFAULT_ARCH), get("padding_type", "reflect-start"),
-                    float(get("tanh_constant", 150.0)), norm="instance" if int(get("use_instance_norm", 1)) == 1 else "batch")
+                    float(get("tanh_constant", 150.0)), norm="instance" if int(get("use_instance_norm", 1)) == 1 else "batch",
+                    precision=get("precision", "pair"))
 
 
 def synthetic_model(style: str = "candy", arch: str = synth.DEFAULT_ARCH, in_dim: int = 7, norm: str = "instance") -> StyleNet:

@@ -43,6 +43,8 @@ def build_parser():
     a("-style_weights", default="1.0"); a("-style_layers", default="4,9,16,23"); a("-style_target_type", default="gram", choices=["gram", "mean"])
     a("-pipeline", type=int, default=1)  # 1: threaded decode / encode around the host-buffer session (f-2); 0: synchronous driver
     a("-arch", default=core.synth.DEFAULT_ARCH)
+    # not a reference option: "fp16" runs every convolution of the nets in one fp16 pass (fav_net_set_precision)
+    a("-precision", default="pair", choices=["pair", "fp16"])
     return p
 
 
@@ -246,6 +248,7 @@ def run_native(opt, model_vid=None, model_img=None, n_decode=None, n_encode=None
     model = model_vid if model_vid is not None else core.load_model(opt.model_vid, opt.arch)
     if model_img is None and opt.model_img not in ("self", "", None):
         model_img = core.load_model(opt.model_img, opt.model_img_arch or opt.arch, in_dim=3)
+    core.set_precision(opt, model, model_img)
     sess = session.Session(model, H, W)
     if model_img is not None:
         sess.set_image_model(model_img)
@@ -291,6 +294,7 @@ def run_pipelined(opt, depth: int = 8, n_decode: int = 6, n_encode: int = 12, mo
     model = model_vid if model_vid is not None else core.load_model(opt.model_vid, opt.arch)
     if model_img is None and opt.model_img not in ("self", "", None):
         model_img = core.load_model(opt.model_img, opt.model_img_arch or opt.arch, in_dim=3)
+    core.set_precision(opt, model, model_img)
     sess = session.Session(model, H, W)
     if model_img is not None:
         sess.set_image_model(model_img)

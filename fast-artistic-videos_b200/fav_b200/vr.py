@@ -94,6 +94,8 @@ def build_parser():
     # read by func_eval (:408-424) but never declared by the VR script; train_video.lua:33's option and default
     a("-reliable_map_min_filter", type=int, default=7)
     a("-arch", default=core.synth.PAPER_ARCH)
+    # not a reference option: "fp16" runs every convolution of the nets in one fp16 pass (fav_net_set_precision)
+    a("-precision", default="pair", choices=["pair", "fp16"])
     return p
 
 

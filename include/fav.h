@@ -205,8 +205,19 @@ FAV_API int fav_net_param_info(const fav_net_t *net, int index, char *name_out, 
 FAV_API int fav_net_set_param(fav_net_t *net, const char *name, const float *host_data, int64_t numel);
 /* upload + repack weights for the tensor-core path; must be called once after all set_param calls */
 FAV_API int fav_net_finalize(fav_net_t *net);
-/* conv implementation: 0 = tensor-core (wgmma) implicit GEMM (default), 1 = CUDA-core debug comparator */
+/* conv implementation: 0 = tensor-core (wgmma) implicit GEMM (default), 1 = CUDA-core debug comparator.  The comparator
+ * always computes in exact fp32, whatever fav_net_set_precision says. */
 FAV_API int fav_net_set_conv_impl(fav_net_t *net, int impl);
+/* Precision of the stylization net's tensor-core convolutions.  An addition: the reference computes in fp32 only.
+ *   "pair" (default): every operand is an fp16 pair hi + lo and each K step runs three MMAs (hi*hi + lo*hi + hi*lo), fp32
+ *          accumulation: fp32 parity.
+ *   "fp16": single pass, one MMA per K step on the fp16 hi halves (activations rounded to fp16, weights as packed), fp32
+ *          accumulation.  Faster; a deprocessed [0,1] frame moves by about one 8-bit level (DESIGN.md §2).  Not
+ *          bit-comparable with "pair": a recurrent clip drifts apart from the exact one within tens of frames.
+ * Anything else: FAV_ERR_INVALID.  A change drops the net's cached plans and CUDA graphs; the next call rebuilds them in the
+ * new mode.  Finish every frame in flight on the net first (fav_session_sync for a session).  Neither the CUDA-core
+ * comparator nor the loss network (fav_percep_*) is affected. */
+FAV_API int fav_net_set_precision(fav_net_t *net, const char *mode);
 /* model:forward(input)                          fast_artistic_video_core.lua:138,172
  * in7 [in_dim,H,W] device fp32 -> out3 [3,H,W] device fp32 in net space (before deprocess). */
 FAV_API int fav_net_forward(fav_net_t *net, const float *in7, int H, int W, float *out3, void *stream);
