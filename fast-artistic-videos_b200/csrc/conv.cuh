@@ -128,6 +128,14 @@ struct ConvJob {
   // MMA per K step on the hi halves alone.  The operands and weights are the same; a single-pass launch copies and reads only
   // their hi planes (the lo halves of the stages and weight slots go unused).  Picks the conv_tc_kernel instance.
   int single;
+  // style bank (fav_net_add_style): image b runs with style img_style[b], a device table the caller writes before each launch
+  // (null: every image runs style 0, the fields below are unused).  Style s's packed weights start s * b_style16 16-byte units
+  // after b, its bias and epi_scale s * bias_style floats after theirs, its nl_gamma / nl_beta s * nl_style floats after theirs,
+  // and its 2^-w_exp is w_unscale_style[s].  Only the batched kernel instances read them (style_at).
+  const int *img_style;
+  const float *w_unscale_style;
+  int64_t b_style16;
+  int bias_style, nl_style;
 };
 
 // Bytes conv_tc_kernel's producers announce on a full barrier (mbarrier expect-tx): they must equal what the bulk copies land
@@ -162,6 +170,31 @@ __host__ __device__ inline TileAt tile_at(const ConvJob &j, int T, bool batch = 
   a.nl_raw4 = a.b * j.nl_raw_img4; a.nl_sums = a.b * j.nl_sums_img;
   return a;
 }
+
+// The parameters image b of a batched job runs with: its style's packed weights, bias, 2^-w_exp, norm-on-load gamma / beta and
+// operand-epilogue scale (ConvJob::img_style).  Shared by the consumers, the weight producer and the norm-on-load producers of
+// conv_tc_kernel's batched instances and by the CPU emulator (tests/emu/style_bank_emu.cu); a single-image launch of a net
+// with one style uses the job's own pointers.
+struct StyleAt {
+  const uint4 *b;
+  const float *bias, *epi_scale, *nl_gamma, *nl_beta;
+  float w_unscale;
+};
+__host__ __device__ inline StyleAt style_at(const ConvJob &j, int b) {
+  StyleAt s{j.b, j.bias, j.epi_scale, j.nl_gamma, j.nl_beta, j.w_unscale};
+  if (!j.img_style) return s;
+  const int st = j.img_style[b];
+  s.b += st * j.b_style16;
+  s.bias += (int64_t)st * j.bias_style;
+  if (s.epi_scale) s.epi_scale += (int64_t)st * j.bias_style;
+  if (s.nl_gamma) { s.nl_gamma += (int64_t)st * j.nl_style; s.nl_beta += (int64_t)st * j.nl_style; }
+  s.w_unscale = j.w_unscale_style[st];
+  return s;
+}
+
+// Whether a job's weights may stay resident in shared memory (conv_tc_choose_slots): loaded once per CTA, they serve every tile
+// the CTA runs, and a banked job's CTAs run tiles of images of different styles.  Shared with the CPU emulator.
+__host__ __device__ inline bool tc_may_keep_weights(const ConvJob &j) { return !j.img_style; }
 
 // Operand epilogue addressing, shared by conv_tc_kernel and its CPU emulators (tests/emu/opnd_epi_emu.cu, batch_emu.cu).  tile:
 // the batched tile index T of tile_at.  Consumer thread t (0..255) of a tile holds, for i < Npad / 8 and h < 2, the accumulator pair of channels c, c + 1 (c = 8i + 2 (t % 4)) of tile
@@ -256,12 +289,14 @@ void conv_tc_choose_slots(ConvJob &job);  // fills b_slots / b_resident from the
 int launch_pack_input(const float *in, int Cin, int H, int W, int reflect, const Operand &dst, cudaStream_t st, int nimg = 1);
 int launch_in_stats(const RawTensor &raw, double *sums /*[2*C]*/, cudaStream_t st, int nimg = 1, int64_t sums_img = 0);
 // sums == null: no normalisation (batch-normalized nets on the CUDA-core comparator: ReLU / skip / pack only)
+// styles non-null (a net with a style bank): image b reads its parameters styles[b] * param_style floats further in
 int launch_in_apply(const RawTensor &raw, const double *sums, const float *gamma, const float *beta, float eps, int relu,
-                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st, int nimg = 1, int64_t sums_img = 0);
+                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st, int nimg = 1, int64_t sums_img = 0,
+                    const int *styles = nullptr, int64_t param_style = 0);
 // tab_mean / tab_scale non-null: a fixed per-channel affine (inference-mode BatchNorm) instead of the statistics of src
 int launch_up_in(const Operand &src, double *sums, const float *gamma, const float *beta, float eps, int relu, int scale,
                  const Operand &dst, cudaStream_t st, const float *tab_mean = nullptr, const float *tab_scale = nullptr,
-                 int nimg = 1, int64_t sums_img = 0);
+                 int nimg = 1, int64_t sums_img = 0, const int *styles = nullptr, int64_t param_style = 0);
 int launch_unpack_operand(const Operand &src, float *out_nchw, cudaStream_t st);
 
 }  // namespace fav

@@ -136,6 +136,10 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
     // gets when it runs alone (DESIGN.md 4.1)
     const TileAt img = tile_at(job, tile, BATCH);
     const int img_end = min(total, (img.b + 1) * job.ntiles);
+    // the bias and scales of this image's style (style_at): the images of a batch may run different weight sets.  A single
+    // image reads the job's own (written out at each use, which keeps the code of those instances as it was)
+    StyleAt sty{};
+    if constexpr (BATCH) sty = style_at(job, img.b);
     for (; tile < img_end; tile += gridDim.x, ++tl) {
       if (job.b_resident) sb = 0;
       uint32_t scale = 0;
@@ -187,7 +191,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
       // 2^w_exp: every store takes acc * 2^-w_exp (exact) before the bias =====
       const TileAt at = tile_at(job, tile, BATCH);  // y, x0; the image's offsets are img's
       const int x0 = at.x0, y = at.y, yo = y * job.oy_mul + job.oy_off;
-      const float ws = OPND ? 1.f : job.w_unscale;  // the operand epilogue's epi_scale includes it
+      const float ws = OPND ? 1.f : (BATCH ? sty.w_unscale : job.w_unscale);  // the operand epilogue's epi_scale includes it
       if (job.xfold_kw) {
         // partial sums Q[pixel][kx*Cout + co] -> shared memory, then out[x][co] = sum_kx Q[x + kx][kx*Cout + co]
         const int ncol = job.xfold_kw * job.Cout;
@@ -207,7 +211,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
           const float *qv = exch + px * kExchPitch;
           const int64_t plane = (int64_t)job.Ho * job.Wo, o = (int64_t)yo * job.Wo + xo;
           for (int k = 0; k < job.Cout; ++k) {
-            float sum = __ldg(job.bias + k);
+            float sum = __ldg((BATCH ? sty.bias : job.bias) + k);
             for (int kx = 0; kx < job.xfold_kw; ++kx) sum += qv[kx * (kExchPitch + job.Cout) + k];
             job.out3[img.out3 + (job.final_mode == 2 ? 2 - k : k) * plane + o] = tc_final_value(sum, k, job.final_mode, job.tanh_c);
           }
@@ -232,7 +236,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
             const int k = q2 + e;
             if (k < 3 && k < job.Cout && valid[h])
               job.out3[img.out3 + ((int64_t)(job.final_mode == 2 ? 2 - k : k) * job.Ho + yo) * job.Wo + xo[h]] =
-                  tc_final_value(fmaf(acc[2 * h + e], ws, __ldg(job.bias + k)), k, job.final_mode, job.tanh_c);
+                  tc_final_value(fmaf(acc[2 * h + e], ws, __ldg((BATCH ? sty.bias : job.bias) + k)), k, job.final_mode, job.tanh_c);
           }
         continue;
       }
@@ -244,7 +248,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   #pragma unroll
         for (int i = 0; i < NJ; ++i) {
           const int n = 8 * i + q2;
-          const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + n));  // the bias of each stacked phase
+          const float2 b = __ldg(reinterpret_cast<const float2 *>((BATCH ? sty.bias : job.bias) + n));  // the bias of each stacked phase
           float v[4];
   #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -268,7 +272,8 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
         for (int i = 0; i < NJ; ++i) {
           const int c = 8 * i + q2;
           // bias and scale are padded to Npad; the scale includes the weights' 2^-w_exp (pack_conv_weights, net.cu)
-          const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c)), s = __ldg(reinterpret_cast<const float2 *>(job.epi_scale + c));
+          const float2 b = __ldg(reinterpret_cast<const float2 *>((BATCH ? sty.bias : job.bias) + c)),
+                     s = __ldg(reinterpret_cast<const float2 *>((BATCH ? sty.epi_scale : job.epi_scale) + c));
   #pragma unroll
           for (int h = 0; h < 2; ++h) {
             int64_t o, so;
@@ -296,7 +301,7 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   #pragma unroll
       for (int i = 0; i < NJ; ++i) {
         const int c = 8 * i + q2;
-        const float2 b = __ldg(reinterpret_cast<const float2 *>(job.bias + c));
+        const float2 b = __ldg(reinterpret_cast<const float2 *>((BATCH ? sty.bias : job.bias) + c));
         float v[4];
   #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -315,13 +320,19 @@ __device__ __forceinline__ void tc_consume(const ConvJob &job, uint8_t *a_base, 
   }
 }
 
-// norm-on-load table of image b (threads tid, tid + nthr, ...)
+// norm-on-load table of image b (threads tid, tid + nthr, ...), with the gamma / beta of its style (style_at)
+template <bool BATCH>
 __device__ __forceinline__ void nl_build_table(const ConvJob &job, float *nl_tab, int b, int tid, int nthr) {
   const double *sums = job.nl_sums + b * job.nl_sums_img;
+  const float *gamma = job.nl_gamma, *beta = job.nl_beta;
+  if constexpr (BATCH) {
+    const StyleAt sty = style_at(job, b);
+    gamma = sty.nl_gamma; beta = sty.nl_beta;
+  }
 #pragma unroll 1  // kept rolled: an unrolled copy inside the producer loop costs the OPND instances a 4-byte spill
   for (int c = tid; c < job.nl_C; c += nthr) {
-    in_finalize(sums[c], sums[job.nl_C + c], job.nl_inv_count, job.nl_eps, job.nl_gamma[c], nl_tab[c], nl_tab[kNlMaxC + c]);
-    nl_tab[2 * kNlMaxC + c] = job.nl_beta[c];
+    in_finalize(sums[c], sums[job.nl_C + c], job.nl_inv_count, job.nl_eps, gamma[c], nl_tab[c], nl_tab[kNlMaxC + c]);
+    nl_tab[2 * kNlMaxC + c] = beta[c];
   }
 }
 
@@ -357,7 +368,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   float *nl_tab = exch + (job.xfold_kw ? kTileM * kExchPitch : 256 + 8 * 2 * 128);
   const int total = (BATCH ? job.nimg : 1) * job.ntiles;
   int nl_b = BATCH ? (int)blockIdx.x / job.ntiles : 0;  // image whose statistics nl_tab holds
-  if (job.nl) nl_build_table(job, nl_tab, nl_b, threadIdx.x, blockDim.x);
+  if (job.nl) nl_build_table<BATCH>(job, nl_tab, nl_b, threadIdx.x, blockDim.x);
   __syncthreads();
   if (threadIdx.x == 0 && job.trace) trace_put(job, 2, clock64());
 
@@ -377,10 +388,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
       const TileAt at = tile_at(job, tile, BATCH);
       const int y = at.y, x0 = at.x0;
       if (at.b != nl_b) {
-        // the next image: its table replaces the current one once all producer warps are done with the previous tile
+        // the next image (and its style): its table replaces the current one once all producer warps are done with the
+        // previous tile
         nl_b = at.b;
         asm volatile("bar.sync 2, %0;" ::"r"(32 * kNlWarps) : "memory");
-        nl_build_table(job, nl_tab, nl_b, threadIdx.x - kAWarp * 32, 32 * kNlWarps);
+        nl_build_table<BATCH>(job, nl_tab, nl_b, threadIdx.x - kAWarp * 32, 32 * kNlWarps);
         asm volatile("bar.sync 2, %0;" ::"r"(32 * kNlWarps) : "memory");
       }
       const float4 *nl_raw = job.nl_raw + at.nl_raw4;
@@ -471,17 +483,19 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
       }
     }
   } else if (warp == kBWarp) {
-    // ===== B producer: weight chunks (the hi steps, the first half of each chunk, only: !PAIR) =====
+    // ===== B producer: weight chunks (the hi steps, the first half of each chunk, only: !PAIR), from the style of the tile's
+    // image (style_at; a net with several styles streams every job's weights, conv_tc_choose_slots) =====
     if (lane == 0) {
       uint32_t s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
         if (job.b_resident && tile != (int)blockIdx.x) break;  // resident weights: one pass fills every slot
+        const uint4 *wb = BATCH ? style_at(job, tile_at(job, tile).b).b : job.b;
         for (int g = 0; g < ngroups; ++g)
           for (int c = 0; c < nchunks; ++c) {
             mbar_wait(&sh->b_empty[s], ph ^ 1);
             const uint32_t cb = FAV_TC_B_CHUNK_TX(job.dbg, chunk_bytes, PAIR);
             mbar_arrive_expect_tx(&sh->b_full[s], cb);
-            bulk_g2s(b_base + s * chunk_bytes, job.b + (int64_t)(g * nchunks + c) * job.chunk16, cb, &sh->b_full[s]);
+            bulk_g2s(b_base + s * chunk_bytes, wb + (int64_t)(g * nchunks + c) * job.chunk16, cb, &sh->b_full[s]);
             if (++s == nslots) { s = 0; ph ^= 1; }
           }
       }
@@ -525,7 +539,8 @@ void conv_tc_choose_slots(ConvJob &job) {
     if (n >= 2 && n <= kMaxA && tc_fixed_smem(t) + 2 * chunk <= budget) job.a_stages = n;
   }
   const size_t fixed = tc_fixed_smem(job);
-  if (total <= kMaxB && fixed + total * chunk <= budget) {
+  // a banked job streams its chunks through the ring, per tile from the tile's style (tc_may_keep_weights)
+  if (total <= kMaxB && fixed + total * chunk <= budget && tc_may_keep_weights(job)) {
     job.b_resident = 1;
     job.b_slots = total;
   } else {
@@ -554,7 +569,8 @@ int launch_conv_tc(const ConvJob &job_in, int num_sms, cudaStream_t st) {
     return FAV_ERR_UNSUPPORTED;
   }
   void (*kernel)(ConvJob) = nullptr;
-  const bool batch = job.nimg > 1, pair = !job.single;
+  // a job with a style table runs the batched instances for one image too: they look the image's style up (style_at)
+  const bool batch = job.nimg > 1 || job.img_style, pair = !job.single;
 #define FAV_TC_PICK(N, P)                                                                                      \
   (job.opnd ? (batch ? conv_tc_kernel<N, true, true, P> : conv_tc_kernel<N, true, false, P>)                   \
             : (batch ? conv_tc_kernel<N, false, true, P> : conv_tc_kernel<N, false, false, P>))

@@ -123,6 +123,10 @@ struct Plan {
   // -scale_factor (fav_run_image_scaled): the content resampled to this plan's size, allocated on the first such call
   float *scaled_in = nullptr;
   std::vector<PlanStep> steps;
+  // a net with a style bank (fav_net_add_style): the style of each image, read by every batched kernel (ConvJob::img_style),
+  // and the assignment it holds, which bind_styles rewrites on the call's stream when it changes; null with one style
+  int *styles = nullptr;
+  std::vector<int> styles_host;
   std::map<int, int> layer_operand;  // arch token index -> operand holding its output
   // CUDA graphs of the whole per-frame kernel sequence (run_[next_]image), one per destination buffer: a frame is ~40
   // launches and the host needs ~1.1 ms to enqueue them one by one (measured, bench e2e), about the GPU time itself
@@ -160,6 +164,13 @@ struct fav_net {
   std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>> plans;  // (B, H, W)
   Plan *last_plan = nullptr;
   size_t budget = kMaxPlanBytes;  // activation bytes of plans created from now on (fav_net_set_activation_budget)
+  // style bank (fav_net_add_style): every parameter buffer holds nstyles copies, bank[buffer] bytes apart (style 0: the net's
+  // own parameters); d_unscale[conv]: 2^-w_exp of each style (kMaxBatch floats, allocated by the first add_style).
+  // batch_styles: the style of each image of later calls (fav_net_set_batch_styles), empty = style 0 for every image
+  int nstyles = 1;
+  std::map<const void *, size_t> bank;
+  std::vector<float *> d_unscale;
+  std::vector<int> batch_styles;
   std::vector<void *> allocs;
   ~fav_net() {
     plans.clear();
@@ -209,11 +220,14 @@ static int add_in(fav_net *net, const std::string &name, int C, int conv) {
   return (int)net->inorms.size() - 1;
 }
 
+// a parameter buffer of one style: its size rounded up to 256 bytes is the stride of its style bank (fav_net_add_style)
 template <class T>
 static int dev_upload(fav_net *net, const std::vector<T> &h, T **out) {
   void *d = nullptr;
-  FAV_TRY(check_cuda(cudaMalloc(&d, std::max<size_t>(h.size() * sizeof(T), 16)), "cudaMalloc(weights)"));
+  const size_t bytes = (std::max<size_t>(h.size() * sizeof(T), 16) + 255) / 256 * 256;
+  FAV_TRY(check_cuda(cudaMalloc(&d, bytes), "cudaMalloc(weights)"));
   net->allocs.push_back(d);
+  net->bank[d] = bytes;
   FAV_TRY(check_cuda(cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice), "cudaMemcpy(weights)"));
   *out = (T *)d;
   return FAV_OK;
@@ -352,6 +366,16 @@ static int make_operand(Plan &pl, int C, int H, int W, const ConvDef *consumer, 
   return FAV_OK;
 }
 
+// a job of conv `conv` in a plan with a style table: image b runs the weights, bias, epilogue scale and 2^-w_exp of style
+// pl.styles[b] (style_at, conv.cuh).  The bias and the epilogue scale are both Npad floats, so one stride serves both.
+static void set_job_styles(const fav_net *net, const Plan &pl, ConvJob &j, int conv) {
+  if (!pl.styles) return;
+  j.img_style = pl.styles;
+  j.w_unscale_style = net->d_unscale[conv];
+  j.b_style16 = (int64_t)(net->bank.at(j.b) / 16);
+  j.bias_style = (int)(net->bank.at(j.bias) / 4);
+}
+
 // tensor-core jobs of c (one per phase, per N block when Cout > kMaxNBlock, or the stacked-phase jobs of plan_phase_stack) and
 // CUDA-core comparator jobs (one per phase); stats: the [sum][sum of squares] slots of c's output for the fused InstanceNorm
 // statistics, or null; epi (batch-normalized nets): the operand step whose ReLU / skip / packing the tensor-core epilogue
@@ -377,6 +401,7 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
           j.final_mode = 0; j.out3 = out3; j.tanh_c = net->tanh_c;
           conv_nblock_stats(j, stats, c.cout, b);
           j.single = net->single;
+          set_job_styles(net, pl, j, (int)(&c - net->convs.data()));
           conv_tc_choose_slots(j);
           if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
           if (conv_tc_smem_bytes(j) > 227 * 1024) { set_error("conv %s: shared memory budget exceeded (fold)", c.name.c_str()); return FAV_ERR_UNSUPPORTED; }
@@ -393,6 +418,7 @@ static int build_conv_jobs(fav_net *net, Plan &pl, PlanStep &st, const ConvDef &
         if (epi)
           set_opnd_epilogue(j, b, cd.d_scale, pl.ops[epi->dst], epi->relu, epi->skip >= 0 ? &pl.ops[epi->skip] : nullptr, epi->shave);
         j.single = net->single;  // the norm-on-load copies (fuse_norm_on_load) and tc_plain keep it
+        set_job_styles(net, pl, j, (int)(&c - net->convs.data()));
         conv_tc_choose_slots(j);
         if (const char *e = getenv("FAV_DBG")) j.dbg = atoi(e);
         if (conv_tc_smem_bytes(j) > 227 * 1024) {
@@ -438,6 +464,7 @@ static void fuse_norm_on_load(fav_net *net, Plan &pl, PlanStep &cs, bool src_is_
     if (!nl_geometry_ok(j) || j.xfold_kw) return;
     ConvJob t = j;
     set_norm_on_load(t, ap.raw, pl.ops[cs.src], ap.relu, pl.stats + ap.stats_off, pl.stats_img, n.d_gamma, n.d_beta);
+    if (t.img_style) t.nl_style = (int)(net->bank.at(n.d_gamma) / 4);
     conv_tc_choose_slots(t);
     if (conv_tc_smem_bytes(t) > 227 * 1024 || !(t.b_resident || t.b_slots >= 2)) return;
     fused.push_back(t);
@@ -649,6 +676,12 @@ static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
     }
     pl->kept = ap.kept;
   }
+  if (net->nstyles > 1) {
+    FAV_TRY(check_cuda(cudaMalloc(&pl->styles, kMaxBatch * sizeof(int)), "cudaMalloc(style table)"));
+    pl->allocs.push_back(pl->styles);
+    FAV_TRY(check_cuda(cudaMemset(pl->styles, 0, kMaxBatch * sizeof(int)), "cudaMemset(style table)"));
+    pl->styles_host.assign(B, 0);
+  }
   FAV_TRY(build_plan_steps(net, pl.get()));
   if (pl->arena) {
     for (size_t i = 0; i < pl->ops.size(); ++i) {
@@ -660,6 +693,23 @@ static int build_plan(fav_net *net, int B, int H, int W, Plan **out) {
   *out = pl.get();
   net->last_plan = pl.get();
   net->plans[key] = std::move(pl);
+  return FAV_OK;
+}
+
+// The plan of a call on B frames of H x W, with its style table holding the net's batch assignment (fav_net_set_batch_styles),
+// written on the call's stream when it changed: the plan and its CUDA graphs stay as they are.
+static int plan_for_call(fav_net *net, int B, int H, int W, cudaStream_t st, Plan **out) {
+  const std::vector<int> &a = net->batch_styles;
+  FAV_REQUIRE(a.empty() || (int)a.size() == B, "a call on %d frames with a style assignment for %d (fav_net_set_batch_styles): the "
+              "batch must have one frame per entry, or the assignment must be cleared (n = 0)", B, (int)a.size());
+  FAV_TRY(build_plan(net, B, H, W, out));
+  Plan &pl = **out;
+  if (!pl.styles) return FAV_OK;
+  const std::vector<int> want = a.empty() ? std::vector<int>(B, 0) : a;
+  if (want == pl.styles_host) return FAV_OK;
+  // pageable source: staged before the call returns, ordered on st before the frame's kernels
+  FAV_TRY(check_cuda(cudaMemcpyAsync(pl.styles, want.data(), B * sizeof(int), cudaMemcpyHostToDevice, st), "cudaMemcpyAsync(styles)"));
+  pl.styles_host = want;
   return FAV_OK;
 }
 
@@ -729,8 +779,13 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
       } else {
         for (SimtJob &j : s.simt) {
           if (j.final_mode) { j.final_mode = final_mode; j.out3 = out3; }
-          for (int b = 0; b < pl.B; ++b) {  // the comparator runs one image at a time
+          for (int b = 0; b < pl.B; ++b) {  // the comparator runs one image at a time, with its style's weights and bias
             SimtJob jb = j;
+            if (pl.styles) {
+              const int sb = pl.styles_host[b];
+              jb.w += sb * (int64_t)(net->bank.at(j.w) / 4);
+              jb.bias += sb * (int64_t)(net->bank.at(j.bias) / 4);
+            }
             jb.in = image_of(j.in, b);
             jb.raw = j.raw ? j.raw + b * s.raw.img : nullptr;
             jb.out3 = j.out3 ? j.out3 + (int64_t)b * 3 * pl.H * pl.W : nullptr;
@@ -744,7 +799,7 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
       const Operand &src = pl.ops[s.src];
       FAV_TRY(begin(3, 12.0 * n.C * src.H * src.W * (1.0 + s.scale * s.scale) / 2.0, n.name + ".up"));
       FAV_TRY(launch_up_in(src, pl.stats + s.stats_off, n.d_gamma, n.d_beta, 1e-5f, s.relu, s.scale, pl.ops[s.dst], st, n.d_mean,
-                           n.d_scale, pl.B, pl.stats_img));
+                           n.d_scale, pl.B, pl.stats_img, pl.styles, pl.styles ? (int64_t)(net->bank.at(n.d_beta) / 4) : 0));
       FAV_TRY(end());
     } else {
       if (s.fused_nl && net->conv_impl == 0 && !unfused) continue;  // the consumer conv normalises while it loads (norm-on-load)
@@ -767,7 +822,8 @@ static int run_plan(fav_net *net, Plan &pl, const float *in7, float *out3, int f
       // InstanceNormalization.lua:21,39: eps = 1e-5, statistics over H*W of each (n, c)
       FAV_TRY(begin(3, (s.skip >= 0 ? 12.0 : 8.0) * elems, n.name + ".apply"));
       FAV_TRY(launch_in_apply(s.raw, sums, n.d_gamma, n.d_beta, 1e-5f, s.relu, s.skip >= 0 ? &pl.ops[s.skip] : nullptr, s.shave,
-                              pl.ops[s.dst], st, pl.B, pl.stats_img));
+                              pl.ops[s.dst], st, pl.B, pl.stats_img, pl.styles,
+                              pl.styles ? (int64_t)(net->bank.at(n.d_gamma) / 4) : 0));
       FAV_TRY(end());
     }
   }
@@ -1027,6 +1083,106 @@ int fav_net_set_precision(fav_net_t *net, const char *mode) {
   return FAV_OK;
 }
 
+// Every device parameter buffer of a finalized net, in one fixed order (null where the net has no such buffer): the
+// buffers a style bank holds one copy of per style
+static std::vector<void **> bank_slots(fav_net *net) {
+  std::vector<void **> v;
+  auto add = [&v](auto *&p) { v.push_back(reinterpret_cast<void **>(&p)); };
+  for (ConvDef &c : net->convs) {
+    add(c.d_bias); add(c.d_scale); add(c.d_stack_bias);
+    for (ConvPhase &ph : c.phases) { add(ph.d_w_simt); add(ph.d_b_tc); }
+    for (ConvPhase &ph : c.stack) add(ph.d_b_tc);
+    for (ConvDef &cb : c.nblock) {
+      add(cb.d_bias); add(cb.d_scale);
+      for (ConvPhase &ph : cb.phases) add(ph.d_b_tc);
+    }
+  }
+  for (InDef &n : net->inorms) { add(n.d_gamma); add(n.d_beta); add(n.d_mean); add(n.d_scale); }
+  return v;
+}
+
+// Style S of net = style 0 of src: each bank buffer grows by one copy of src's (a new allocation: the S styles it held, then
+// src's), every pointer of the net moves to its new bank, and the plans built for S styles are dropped.
+int fav_net_add_style(fav_net_t *net, const fav_net_t *src, int *index_out) {
+  FAV_REQUIRE(net && src && index_out, "fav_net_add_style: null argument");
+  FAV_REQUIRE(net->finalized && src->finalized, "fav_net_add_style: both nets must be finalized (fav_net_finalize)");
+  FAV_REQUIRE(net != src, "fav_net_add_style: a net cannot add itself");
+  FAV_REQUIRE(net->arch == src->arch, "fav_net_add_style: the nets differ in arch ('%s' and '%s')", net->arch.c_str(), src->arch.c_str());
+  FAV_REQUIRE(net->padding_type == src->padding_type, "fav_net_add_style: the nets differ in padding_type ('%s' and '%s')",
+              net->padding_type.c_str(), src->padding_type.c_str());
+  FAV_REQUIRE(net->tanh_c == src->tanh_c, "fav_net_add_style: the nets differ in tanh_constant (%g and %g)", net->tanh_c, src->tanh_c);
+  FAV_REQUIRE(net->in_dim == src->in_dim, "fav_net_add_style: the nets differ in in_dim (%d and %d)", net->in_dim, src->in_dim);
+  FAV_REQUIRE(net->bn == src->bn, "fav_net_add_style: the nets differ in norm ('%s' and '%s')", net->bn ? "batch" : "instance",
+              src->bn ? "batch" : "instance");
+  FAV_REQUIRE(net->device == src->device, "fav_net_add_style: the nets live on devices %d and %d", net->device, src->device);
+  FAV_REQUIRE(net->nstyles < kMaxBatch, "fav_net_add_style: a net holds at most %d styles (the batch limit)", kMaxBatch);
+  const int S = net->nstyles;
+  if (net->d_unscale.empty()) {
+    for (const ConvDef &c : net->convs) {
+      float *d = nullptr;
+      FAV_TRY(check_cuda(cudaMalloc(&d, kMaxBatch * sizeof(float)), "cudaMalloc(style unscale)"));
+      net->allocs.push_back(d);
+      net->d_unscale.push_back(d);
+      const float u = ldexpf(1.f, -c.w_exp);
+      FAV_TRY(check_cuda(cudaMemcpy(d, &u, sizeof(float), cudaMemcpyHostToDevice), "cudaMemcpy(style unscale)"));
+    }
+  }
+  std::vector<void **> to = bank_slots(net), from = bank_slots(const_cast<fav_net *>(src));
+  // allocate every grown bank first: a failure leaves the net as it was
+  std::vector<void *> grown(to.size(), nullptr);
+  int rc = FAV_OK;
+  for (size_t i = 0; i < to.size() && rc == FAV_OK; ++i) {
+    if ((*to[i] == nullptr) != (*from[i] == nullptr) || (*to[i] && net->bank.at(*to[i]) != src->bank.at(*from[i]))) {
+      set_error("fav_net_add_style: internal: parameter buffer %zu differs in size", i);
+      rc = FAV_ERR_INVALID;
+    } else if (*to[i]) {
+      rc = check_cuda(cudaMalloc(&grown[i], (S + 1) * net->bank.at(*to[i])), "cudaMalloc(style bank)");
+    }
+  }
+  for (size_t i = 0; i < to.size() && rc == FAV_OK; ++i) {
+    if (!*to[i]) continue;
+    const size_t per = net->bank.at(*to[i]);
+    rc = check_cuda(cudaMemcpy(grown[i], *to[i], S * per, cudaMemcpyDeviceToDevice), "cudaMemcpy(style bank)");
+    if (rc == FAV_OK)
+      rc = check_cuda(cudaMemcpy((char *)grown[i] + S * per, *from[i], per, cudaMemcpyDeviceToDevice), "cudaMemcpy(style bank)");
+  }
+  for (size_t c = 0; c < net->convs.size() && rc == FAV_OK; ++c) {
+    const float u = ldexpf(1.f, -src->convs[c].w_exp);
+    rc = check_cuda(cudaMemcpy(net->d_unscale[c] + S, &u, sizeof(float), cudaMemcpyHostToDevice), "cudaMemcpy(style unscale)");
+  }
+  if (rc != FAV_OK) {
+    for (void *p : grown) cudaFree(p);
+    return rc;
+  }
+  net->plans.clear();
+  net->last_plan = nullptr;
+  for (size_t i = 0; i < to.size(); ++i) {
+    if (!*to[i]) continue;
+    const size_t per = net->bank.at(*to[i]);
+    net->bank.erase(*to[i]);
+    net->allocs.erase(std::find(net->allocs.begin(), net->allocs.end(), *to[i]));
+    cudaFree(*to[i]);
+    *to[i] = grown[i];
+    net->bank[grown[i]] = per;
+    net->allocs.push_back(grown[i]);
+  }
+  net->nstyles = S + 1;
+  *index_out = S;
+  return FAV_OK;
+}
+
+int fav_net_num_styles(const fav_net_t *net) { return net ? net->nstyles : 0; }
+
+int fav_net_set_batch_styles(fav_net_t *net, const int *styles, int n) {
+  FAV_REQUIRE(net && (n == 0 || styles), "fav_net_set_batch_styles: null argument");
+  FAV_REQUIRE(n >= 0 && n <= kMaxBatch, "fav_net_set_batch_styles: %d entries; a batch has 1 to %d frames (0 clears)", n, kMaxBatch);
+  for (int i = 0; i < n; ++i)
+    FAV_REQUIRE(styles[i] >= 0 && styles[i] < net->nstyles, "fav_net_set_batch_styles: image %d gets style %d; the net holds %d",
+                i, styles[i], net->nstyles);
+  net->batch_styles.assign(styles, styles + n);
+  return FAV_OK;
+}
+
 int fav_net_set_activation_budget(fav_net_t *net, size_t bytes) {
   FAV_REQUIRE(net && bytes > 0, "fav_net_set_activation_budget: null net or zero budget");
   net->budget = bytes;
@@ -1050,7 +1206,7 @@ int fav_net_forward_batch(fav_net_t *net, const float *in, int B, int H, int W, 
   FAV_REQUIRE(net && in && out3, "fav_net_forward: null argument");
   FAV_REQUIRE(net->finalized, "fav_net_forward: call fav_net_finalize first");
   Plan *pl;
-  FAV_TRY(build_plan(net, B, H, W, &pl));
+  FAV_TRY(plan_for_call(net, B, H, W, (cudaStream_t)stream, &pl));
   return run_plan(net, *pl, in, out3, 1, (cudaStream_t)stream);
 }
 
@@ -1059,9 +1215,9 @@ int fav_net_profile(fav_net_t *net, const float *in7, int H, int W, float *out3,
   FAV_REQUIRE(net && in7 && out3 && kinds && ms && work && n_out, "fav_net_profile: null argument");
   FAV_REQUIRE(net->finalized, "fav_net_profile: call fav_net_finalize first");
   Plan *pl;
-  FAV_TRY(build_plan(net, 1, H, W, &pl));
-  std::vector<ProfRec> prof;
   cudaStream_t st = (cudaStream_t)stream;
+  FAV_TRY(plan_for_call(net, 1, H, W, st, &pl));
+  std::vector<ProfRec> prof;
   int rc = run_plan(net, *pl, in7, out3, 1, st, &prof);
   if (rc == FAV_OK) rc = check_cuda(cudaStreamSynchronize(st), "fav_net_profile sync");
   int n = 0;
@@ -1126,8 +1282,8 @@ int fav_run_image_batch(fav_net_t *net, const float *content, const float *fill,
   FAV_REQUIRE(net->in_dim == 7 || net->in_dim == 3, "fav_run_image: video model (7 input channels) or image model (3) required");
   if (net->in_dim == 3) fill = nullptr;
   Plan *pl;
-  FAV_TRY(build_plan(net, B, H, W, &pl));
   cudaStream_t st = (cudaStream_t)stream;
+  FAV_TRY(plan_for_call(net, B, H, W, st, &pl));
   static const bool fuse_pack = getenv("FAV_NO_FUSEPACK") == nullptr;
   if (fuse_pack) {
     FAV_TRY(launch_temporal_input_packed(content, nullptr, nullptr, nullptr, fill, nullptr, pl->ops[0], net->reflect_pad, H, W, 0, true, st,
@@ -1156,8 +1312,8 @@ int fav_run_image_scaled(fav_net_t *net, const float *content, int H, int W, dou
   const int h = (int)hd, w = (int)wd;
   FAV_TRY(check_scale_args(content, out_rgb, 3, H, W, h, w));
   Plan *pl;
-  FAV_TRY(build_plan(net, 1, h, w, &pl));  // the frame rules apply at h x w; refusals come before any device work
   cudaStream_t st = (cudaStream_t)stream;
+  FAV_TRY(plan_for_call(net, 1, h, w, st, &pl));  // the frame rules apply at h x w; refusals come before any device work
   // not pl->in7: fav_run_image's unfused path (FAV_NO_FUSEPACK) writes that one
   if (!pl->scaled_in) FAV_TRY(alloc_zero(*pl, (void **)&pl->scaled_in, (size_t)3 * h * w * sizeof(float)));
   FAV_TRY(launch_image_scale_bicubic(content, pl->scaled_in, 3, H, W, h, w, st));
@@ -1181,8 +1337,8 @@ int fav_run_next_image_batch(fav_net_t *net, const float *content, const float *
   FAV_REQUIRE(net->in_dim == 7, "fav_run_next_image: video model (7 input channels) required");
   FAV_REQUIRE(border_mode == FAV_BORDER_PER_TAP || border_mode == FAV_BORDER_PAD_PIXEL, "bad border_mode");
   Plan *pl;
-  FAV_TRY(build_plan(net, B, H, W, &pl));
   cudaStream_t st = (cudaStream_t)stream;
+  FAV_TRY(plan_for_call(net, B, H, W, st, &pl));
   static const bool fuse_pack = getenv("FAV_NO_FUSEPACK") == nullptr;
   if (fuse_pack) {
     FAV_TRY(launch_temporal_input_packed(content, prev_rgb, flow, cert, fill, flow_mask, pl->ops[0], net->reflect_pad, H, W,
@@ -1212,8 +1368,8 @@ int fav_run_next_image_flows_batch(fav_net_t *net, const float *content, const f
   FAV_REQUIRE(border_mode == FAV_BORDER_PER_TAP || border_mode == FAV_BORDER_PAD_PIXEL, "bad border_mode");
   FAV_REQUIRE(min_filter_r >= 0 && (min_filter_r <= 1 || (min_filter_r & 1)) && min_filter_r <= 15, "occlusions_min_filter must be odd <= 15");
   Plan *pl;
-  FAV_TRY(build_plan(net, B, H, W, &pl));
   cudaStream_t st = (cudaStream_t)stream;
+  FAV_TRY(plan_for_call(net, B, H, W, st, &pl));
   static const bool no_stage = getenv("FAV_NO_STAGE") != nullptr;  // A/B timing: the three separate kernels
   int rc = no_stage ? FAV_ERR_UNSUPPORTED
                     : launch_temporal_stage(content, prev_rgb, flow_bw, flow_fw_uv, cert_raw, fill, flow_mask, nullptr, nullptr,
@@ -1257,8 +1413,8 @@ int fav_run_next_image_flows_structure(fav_net_t *net, const float *content, con
   FAV_REQUIRE(border_mode == FAV_BORDER_PER_TAP || border_mode == FAV_BORDER_PAD_PIXEL, "bad border_mode");
   FAV_REQUIRE(min_filter_r >= 0 && (min_filter_r <= 1 || (min_filter_r & 1)) && min_filter_r <= 15, "occlusions_min_filter must be odd <= 15");
   Plan *pl;
-  FAV_TRY(build_plan(net, 1, H, W, &pl));
   cudaStream_t st = (cudaStream_t)stream;
+  FAV_TRY(plan_for_call(net, 1, H, W, st, &pl));
   const int64_t HW = (int64_t)H * W;
   if (!pl->corners_ws) {
     FAV_TRY(alloc_zero(*pl, (void **)&pl->structure, HW * sizeof(float)));

@@ -111,12 +111,14 @@ int launch_in_stats(const RawTensor &raw, double *sums, cudaStream_t st, int nim
 // ---- in_apply ----------------------------------------------------------------------------------------
 // mean / gamma*rstd / beta of the block's 8 channels are derived from the (double) sums by the first 8 threads:
 // biased variance, eps inside the sqrt (nn.SpatialBatchNormalization in training mode, InstanceNormalization.lua:39-50).
-// Batch: blockIdx.z = b * (C / 8) + cb, statistics of image b at sums + b * sums_img.
+// Batch: blockIdx.z = b * (C / 8) + cb, statistics of image b at sums + b * sums_img.  styles (a net with a style bank,
+// fav_net_add_style): image b takes gamma / beta of style styles[b], param_style floats apart; null: style 0.
 template <int ITER>
 __global__ void __launch_bounds__(128) in_apply_kernel(RawTensor raw, const double *__restrict__ sums,
                                                        const float *__restrict__ gamma, const float *__restrict__ beta,
                                                        double inv_count, double eps, int relu, Operand skip, int has_skip,
-                                                       int shave, Operand dst, int64_t sums_img) {
+                                                       int shave, Operand dst, int64_t sums_img, const int *__restrict__ styles,
+                                                       int64_t param_style) {
   __shared__ float s_mean[8], s_scale[8], s_beta[8];
   const int xbase = blockIdx.x * (128 * ITER) + threadIdx.x;
   const int y = blockIdx.y, b = blockIdx.z / (raw.C / 8), cb = blockIdx.z - b * (raw.C / 8);
@@ -152,6 +154,7 @@ __global__ void __launch_bounds__(128) in_apply_kernel(RawTensor raw, const doub
   if (threadIdx.x < 8) {
     int c = cb * 8 + threadIdx.x;
     if (sums) {
+      if (styles) { gamma += styles[b] * param_style; beta += styles[b] * param_style; }
       in_finalize(sums[c], sums[raw.C + c], inv_count, eps, gamma[c], s_mean[threadIdx.x], s_scale[threadIdx.x]);
       s_beta[threadIdx.x] = beta[c];
     } else {
@@ -185,7 +188,8 @@ __global__ void __launch_bounds__(128) in_apply_kernel(RawTensor raw, const doub
 }
 
 int launch_in_apply(const RawTensor &raw, const double *sums, const float *gamma, const float *beta, float eps, int relu,
-                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st, int nimg, int64_t sums_img) {
+                    const Operand *skip, int shave, const Operand &dst, cudaStream_t st, int nimg, int64_t sums_img,
+                    const int *styles, int64_t param_style) {
   // pixels per thread: amortises the per-block finalisation against registers (occupancy); FAV_APPLY_ITER = 2|3|4 for A/B timing
   static const int forced = getenv("FAV_APPLY_ITER") ? atoi(getenv("FAV_APPLY_ITER")) : 0;
   const int iter = forced >= 2 && forced <= 4 ? forced : kApplyIter;
@@ -193,11 +197,14 @@ int launch_in_apply(const RawTensor &raw, const double *sums, const float *gamma
   Operand sk = skip ? *skip : Operand();
   const double inv = 1.0 / ((double)raw.H * raw.W);
   if (iter == 2)
-    in_apply_kernel<2><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img);
+    in_apply_kernel<2><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img,
+                                              styles, param_style);
   else if (iter == 3)
-    in_apply_kernel<3><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img);
+    in_apply_kernel<3><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img,
+                                              styles, param_style);
   else
-    in_apply_kernel<4><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img);
+    in_apply_kernel<4><<<grid, 128, 0, st>>>(raw, sums, gamma, beta, inv, (double)eps, relu, sk, skip ? 1 : 0, shave, dst, sums_img,
+                                              styles, param_style);
   return post_launch("in_apply");
 }
 
@@ -252,7 +259,7 @@ __global__ void __launch_bounds__(128) up_apply_kernel(Operand src, const double
                                                        const float *__restrict__ gamma, const float *__restrict__ beta,
                                                        double inv_count, double eps, int relu, int scale, Operand dst,
                                                        const float *__restrict__ tab_mean, const float *__restrict__ tab_scale,
-                                                       int64_t sums_img) {
+                                                       int64_t sums_img, const int *__restrict__ styles, int64_t param_style) {
   __shared__ float s_mean[8], s_scale[8], s_beta[8];
   const int xbase = blockIdx.x * (128 * kApplyIter) + threadIdx.x;
   const int y = blockIdx.y, b = blockIdx.z / dst.Cb, cb = blockIdx.z - b * dst.Cb;  // batch: blockIdx.z = b * Cb + cb
@@ -260,6 +267,11 @@ __global__ void __launch_bounds__(128) up_apply_kernel(Operand src, const double
   if (sums) sums += b * sums_img;
   if (threadIdx.x < 8) {
     int c = cb * 8 + threadIdx.x;
+    if (styles) {  // style styles[b] of a style bank: its gamma / beta, or its BatchNorm affine
+      const int64_t o = styles[b] * param_style;
+      beta += o;
+      if (tab_scale) { tab_mean += o; tab_scale += o; } else gamma += o;
+    }
     if (tab_scale) {  // inference-mode BatchNorm after the upsampling: running mean, weight / sqrt(running_var + eps)
       s_mean[threadIdx.x] = tab_mean[c]; s_scale[threadIdx.x] = tab_scale[c];
     } else {
@@ -286,14 +298,15 @@ __global__ void __launch_bounds__(128) up_apply_kernel(Operand src, const double
 }
 
 int launch_up_in(const Operand &src, double *sums, const float *gamma, const float *beta, float eps, int relu, int scale,
-                 const Operand &dst, cudaStream_t st, const float *tab_mean, const float *tab_scale, int nimg, int64_t sums_img) {
+                 const Operand &dst, cudaStream_t st, const float *tab_mean, const float *tab_scale, int nimg, int64_t sums_img,
+                 const int *styles, int64_t param_style) {
   if (!tab_scale) {
     opnd_stats_kernel<<<dim3(src.Cb, ceil_div(src.H, kStatRows), nimg), 256, 0, st>>>(src, sums, sums_img);
     FAV_TRY(post_launch("up_in.stats"));
   }
   dim3 grid(ceil_div(dst.W, 128 * kApplyIter), dst.H, dst.Cb * nimg);
   up_apply_kernel<<<grid, 128, 0, st>>>(src, sums, gamma, beta, 1.0 / ((double)src.H * src.W), (double)eps, relu, scale, dst,
-                                        tab_mean, tab_scale, sums_img);
+                                        tab_mean, tab_scale, sums_img, styles, param_style);
   return post_launch("up_in.apply");
 }
 

@@ -112,6 +112,9 @@ SIGNATURES = {
     "fav_net_forward_batch": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]),
     "fav_net_layer_output_image": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _fp, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                              C.POINTER(C.c_int), _fp]),
+    "fav_net_add_style": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
+    "fav_net_num_styles": (C.c_int, [C.c_void_p]),
+    "fav_net_set_batch_styles": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int]),
     "fav_net_set_activation_budget": (C.c_int, [C.c_void_p, C.c_size_t]),
     "fav_net_plan_bytes": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "fav_run_image_batch": (C.c_int, [C.c_void_p, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]),

@@ -214,15 +214,17 @@ def stream_clips(num_clips, n_frames, chunk, in_shapes, out_shape, load_chunk, p
 # bit (models_video.StyleNet batches, include/fav.h fav_run_next_image_batch).
 # ---------------------------------------------------------------------------------------------------------------------
 def run_clips_lockstep(net, frames: torch.Tensor, flows: torch.Tensor, certs: torch.Tensor, fills: Optional[torch.Tensor] = None,
-                       flow_masks: Optional[torch.Tensor] = None, border_mode: int = 0) -> torch.Tensor:
+                       flow_masks: Optional[torch.Tensor] = None, border_mode: int = 0, styles=None) -> torch.Tensor:
     """frames [B,T,3,H,W] RGB in [0,1]; flows [B,T,2,H,W] (dy,dx) and certs [B,T,H,W], entry t used for frame t >= 1 (entry 0 is
     ignored); fills / flow_masks [B,T,3,H,W] / [B,T,H,W] or None.  Frame 0 of every clip goes through run_image (batched),
-    frame t >= 1 through run_next_image on the clips' frames t - 1.  Returns the stylized frames [B,T,3,H,W]."""
+    frame t >= 1 through run_next_image on the clips' frames t - 1.  styles: None, or the style of each clip in net's style bank
+    (StyleNet.add_style): clip b then equals that clip run alone on the net its style came from.  Returns the stylized frames
+    [B,T,3,H,W]."""
     B, T = frames.shape[:2]
     out = torch.empty_like(frames)
     pick = lambda t, i: None if t is None else t[:, i].contiguous()
-    out[:, 0] = net.run_image(frames[:, 0].contiguous(), pick(fills, 0))
+    out[:, 0] = net.run_image(frames[:, 0].contiguous(), pick(fills, 0), styles=styles)
     for i in range(1, T):
         out[:, i] = net.run_next_image(frames[:, i].contiguous(), out[:, i - 1].contiguous(), flows[:, i].contiguous(),
-                                       certs[:, i].contiguous(), pick(fills, i), pick(flow_masks, i), border_mode)
+                                       certs[:, i].contiguous(), pick(fills, i), pick(flow_masks, i), border_mode, styles=styles)
     return out

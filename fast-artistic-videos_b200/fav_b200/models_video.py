@@ -6,6 +6,10 @@ Returns a StyleNet whose `forward(input[Nx7xHxW]) -> [Nx3xHxW]` runs the sm_90a 
 Batches: like the reference nn modules, forward takes N >= 1 images of one size, and run_image / run_next_image /
 run_next_image_flows accept a leading batch dimension.  A batch runs through one plan in one launch per kernel; image b of
 the result is bit-identical to that image run alone.
+
+Style banks (an addition): add_style(other) gives a net further weight sets of its architecture, and `styles=[s_0, ...]` on
+forward / run_image / run_next_image / run_next_image_flows runs image b of a batch with style s_b -- bit-identical to that
+image run alone on the net style s_b came from.
 """
 from __future__ import annotations
 
@@ -79,6 +83,31 @@ class StyleNet:
         _lib.check(_lib.lib.fav_net_set_precision(self._h, mode.encode()))
         self.precision = mode
 
+    def add_style(self, other: "StyleNet") -> int:
+        """Copy other's weights (its style 0) into this net as a new style and return its index (fav_net_add_style).  Both nets
+        must be loaded and agree on arch, padding_type, tanh_constant, in_dim and norm (FavError naming the first that differs);
+        at most 64 styles.  `other` may be dropped afterwards.  The bank runs in this net's precision.  Drops the cached plans
+        and graphs."""
+        idx = C.c_int()
+        _lib.check(_lib.lib.fav_net_add_style(self._h, other._h, C.byref(idx)))
+        return idx.value
+
+    @property
+    def num_styles(self) -> int:
+        """Weight sets this net holds: 1 (its own) plus one per add_style."""
+        return _lib.lib.fav_net_num_styles(self._h)
+
+    def _set_styles(self, styles) -> None:
+        """The style of each image of the next call (fav_net_set_batch_styles); None: style 0 for every image.  A sequence must
+        have one entry per image of that call."""
+        if styles is None:
+            _lib.check(_lib.lib.fav_net_set_batch_styles(self._h, None, 0))
+            return
+        vals = [int(v) for v in styles]
+        if not vals:
+            raise _lib.FavError(_lib.FAV_ERR_INVALID, "styles: an empty sequence (pass None for style 0 everywhere)")
+        _lib.check(_lib.lib.fav_net_set_batch_styles(self._h, (C.c_int * len(vals))(*vals), len(vals)))
+
     def set_activation_budget(self, nbytes: int) -> None:
         """Cap the activation memory of plans (one per batch and frame size) created from now on; default 32 GiB.  A plan
         over the budget shares buffers between layers whose lifetimes do not overlap (same output, bit for bit); one over
@@ -92,13 +121,15 @@ class StyleNet:
         return a.value, s.value
 
     # -- model:forward(input) ----------------------------------------------------------------------
-    def forward(self, input: torch.Tensor) -> torch.Tensor:
+    def forward(self, input: torch.Tensor, styles=None) -> torch.Tensor:
+        """styles: None (style 0), or the style of each of the N images (add_style)."""
         assert input.dim() == 4 and input.size(0) >= 1 and input.size(1) == self.in_dim, \
             f"expected Nx{self.in_dim}xHxW input"
         x = input.contiguous()
         assert x.dtype == torch.float32
         N, (H, W) = x.size(0), x.shape[-2:]
         out = torch.empty((N, 3, H, W), dtype=torch.float32, device=x.device)
+        self._set_styles(styles)
         _lib.check(_lib.lib.fav_net_forward_batch(self._h, _lib.dptr(x), N, H, W, _lib.dptr(out), _lib.stream_ptr()))
         return out
 
@@ -107,6 +138,7 @@ class StyleNet:
         x = input.contiguous()
         H, W = x.shape[-2:]
         out = torch.empty((1, 3, H, W), dtype=torch.float32, device=x.device)
+        self._set_styles(None)
         n_max = 256
         kinds, ms, work = (C.c_int * n_max)(), (C.c_float * n_max)(), (C.c_double * n_max)()
         names = C.create_string_buffer(24 * n_max)
@@ -127,14 +159,16 @@ class StyleNet:
         return out
 
     # -- fused frame-level ops (fast_artistic_video_core.lua:121-180) ------------------------------------
-    def run_image(self, img: torch.Tensor, fill: torch.Tensor = None, scale_factor: float = 1.0) -> torch.Tensor:
-        """img [3,H,W], or [B,3,H,W] for a batch (fill then [B,3,H,W] too).  scale_factor != 1 (-scale_factor, core.lua:127-152):
+    def run_image(self, img: torch.Tensor, fill: torch.Tensor = None, scale_factor: float = 1.0, styles=None) -> torch.Tensor:
+        """img [3,H,W], or [B,3,H,W] for a batch (fill then [B,3,H,W] too).  styles: None (style 0), or one style per image
+        (add_style; one entry for [3,H,W]).  scale_factor != 1 (-scale_factor, core.lua:127-152):
         one image [3,H,W] through an image model (in_dim 3), stylized at (H*sf) x (W*sf) between two bicubic image.scale
         calls (fav_run_image_scaled); fill is then unused, as it is for every image model."""
         x = img.contiguous()
         assert x.dim() in (3, 4) and x.size(-3) == 3 and x.dtype == torch.float32
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
+        self._set_styles(styles)
         if float(scale_factor) != 1:
             if x.dim() != 3:
                 raise _lib.FavError(_lib.FAV_ERR_INVALID, f"run_image with scale_factor {scale_factor}: one image [3,H,W], "
@@ -151,12 +185,14 @@ class StyleNet:
         return out
 
     def run_next_image(self, img, prev_rgb, flow, cert, fill=None, flow_mask=None,
-                       border_mode=_lib.BORDER_PER_TAP) -> torch.Tensor:
+                       border_mode=_lib.BORDER_PER_TAP, styles=None) -> torch.Tensor:
         """img / prev_rgb [3,H,W], flow [2,H,W], cert [H,W]; or all of them (and fill, flow_mask) with a leading batch
-        dimension B: B independent clips advance one frame, each from its own prev_rgb[b]."""
+        dimension B: B independent clips advance one frame, each from its own prev_rgb[b].  styles: None (style 0), or one
+        style per image (add_style)."""
         x = img.contiguous()
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
+        self._set_styles(styles)
         if x.dim() == 3:
             p, f, c = prev_rgb.contiguous(), flow.contiguous(), cert.contiguous()
             _lib.check(_lib.lib.fav_run_next_image(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(c),
@@ -172,13 +208,15 @@ class StyleNet:
 
 
     def run_next_image_flows(self, img, prev_rgb, flow_bw, flow_fw_uv=None, cert_raw=None, min_filter_r=7, fill=None,
-                             flow_mask=None, border_mode=_lib.BORDER_PER_TAP) -> torch.Tensor:
+                             flow_mask=None, border_mode=_lib.BORDER_PER_TAP, styles=None) -> torch.Tensor:
         """run_next_image with func_load_cert + utils.min_filter inside (fav_run_next_image_flows): the whole temporal stage is
         ONE kernel.  flow_bw [2,H,W] (dy,dx); flow_fw_uv [2,H,W] (u,v) -> occlusion test on the GPU, or cert_raw [H,W].
-        A leading batch dimension B on every argument: B independent clips advance one frame."""
+        A leading batch dimension B on every argument: B independent clips advance one frame.  styles: None (style 0), or one
+        style per image (add_style)."""
         x = img.contiguous()
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
+        self._set_styles(styles)
         if x.dim() == 3:
             p, f = prev_rgb.contiguous(), flow_bw.contiguous()
             fw = None if flow_fw_uv is None else flow_fw_uv.contiguous()
@@ -205,6 +243,7 @@ class StyleNet:
         assert x.dim() == 3, "run_next_image_flows_structure: one image [3,H,W]"
         H, W = x.shape[-2:]
         out = torch.empty_like(x)
+        self._set_styles(None)
         p, f, fw = prev_rgb.contiguous(), flow_bw.contiguous(), flow_fw_uv.contiguous()
         _lib.check(_lib.lib.fav_run_next_image_flows_structure(self._h, _lib.dptr(x), _lib.dptr(p), _lib.dptr(f), _lib.dptr(fw),
                                                                _lib.dptr(fill), _lib.dptr(flow_mask), H, W, int(min_filter_r),

@@ -242,8 +242,28 @@ FAV_API int fav_net_layer_output(fav_net_t *net, int index, float *out, int *C, 
  * model:forward(input) of a batch                fast_artistic_video_core.lua:138,172
  * in [B,in_dim,H,W] device fp32 -> out3 [B,3,H,W] device fp32 in net space. */
 FAV_API int fav_net_forward_batch(fav_net_t *net, const float *in, int B, int H, int W, float *out3, void *stream);
-/* fav_net_layer_output for image b of the last forward's batch (models_video.lua:55-140 layer `index`). */
+/* fav_net_layer_output for image b of the last forward's batch (models_video.lua:55-140 layer `index`), computed with the
+ * style that forward gave image b (fav_net_set_batch_styles). */
 FAV_API int fav_net_layer_output_image(fav_net_t *net, int index, int b, float *out, int *C, int *Hl, int *Wl, void *stream);
+
+/* Style banks.  An addition: the reference loads one model per run (fast_artistic_video_core.lua:39-47), and every released
+ * video model (candy, mosaic, ...) has the same architecture (models_video.lua:55-140).  A finalized net can hold S >= 1
+ * weight sets of its own architecture, its styles; style 0 is its own parameters.  A batch may then give each image its own
+ * style: image b of a *_batch call (or fav_net_forward_batch) is bit-identical to the same frame run alone on the net that
+ * style came from.
+ *
+ * fav_net_add_style: style S = src's parameters (its style 0), copied into the net: src may be destroyed afterwards.  Both
+ * nets must be finalized and agree on arch, padding_type, tanh_constant, in_dim and norm (fast_artistic_video_core.lua:39-47
+ * loads them with the checkpoint); otherwise FAV_ERR_INVALID naming the first property that differs.  At most 64 styles (the
+ * batch limit).  *index_out = S.  Drops the net's cached plans and CUDA graphs, as fav_net_set_precision does. */
+FAV_API int fav_net_add_style(fav_net_t *net, const fav_net_t *src, int *index_out);
+/* The number of styles the net holds (1 until fav_net_add_style).  models_video.lua:55-140 builds one. */
+FAV_API int fav_net_num_styles(const fav_net_t *net);
+/* The style of each image of later calls (fast_artistic_video_core.lua:121-180 run_image / run_next_image, batched): image b
+ * runs style styles[b].  n == 0 restores the default, style 0 for every image.  With n > 0 every later forward or run_* call
+ * must have B == n, and each entry must lie in [0, S); otherwise FAV_ERR_INVALID.  A change rebuilds no plan and re-captures
+ * no graph: each call writes the assignment on its own stream before its kernels. */
+FAV_API int fav_net_set_batch_styles(fav_net_t *net, const int *styles, int n);
 
 /* Activation memory.  A plan (one per batch size B and frame size H x W, built at its first call) gives every activation its
  * own buffer when their total fits the net's activation budget.  When it does not, activations whose lifetimes do not overlap
